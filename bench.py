@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — Thor encode on B200: the RD loop of REAL encodes, in Mpixel/s (BASELINE.json metric: "encode Mpixels/s (1080p HDB_high_efficiency)").
+"""bench.py — Thor encode on one GPU: the RD loop of REAL encodes, in Mpixel/s (BASELINE.json metric: "encode Mpixels/s (1080p HDB_high_efficiency)").
 
 WORKLOAD.  A synthetic 4:2:0 clip is encoded ONCE, untimed, by the unmodified reference encoder on the CPU (oracle/_ref/Thorenc_capture: the
 reference's own objects + the observing shim).  The shim writes every frame's RD-loop JOB — the frame parameters the reference chose (type, qp,
@@ -24,6 +24,10 @@ from all of them — the wavefront of one frame is only ~4 super blocks wide, a 
 --impl reference / cpu_baseline: the reference encoder itself (Thorenc_capture) as one process per host thread, all encoding the full-size clip
 continuously; throughput is read in fixed wall-clock slices (one slice = one step) from the progress the observing shim publishes per super block, in
 the encoders' steady state (P + B frames), as pixels decided / seconds inside the reference's process_block loop (the RD loop the GPU arm times).
+
+  --dump-outputs DIR  after the timed steps, the decisions of the last step (the last GOP replica of the end-to-end launch: reconstruction,
+                      block state, RD cost and leaf list per super block) as DIR/<name>.npy, float32/float64, a fixed seeded sample where the
+                      whole would exceed 64 MB; the inputs are the same on every run with the same arguments, so two builds compare output for output
 
   python bench.py --gpus 1 --steps 5 --warmup 3
   python bench.py --impl reference --steps 1 --warmup 0
@@ -160,6 +164,7 @@ class ClockSampler:
     def __init__(self, index=0):
         self.sm, self.mx, self.reasons, self.index = [], [], set(), index
         self.proc, self.thread, self.stop_flag, self.nvml = None, None, threading.Event(), None
+        self.power_limit = None
 
     def _nvml_loop(self):
         import pynvml as nv
@@ -183,13 +188,14 @@ class ClockSampler:
             phys = int(vis.split(",")[self.index]) if vis and all(t.strip().isdigit() for t in vis.split(",")) else self.index
             self.nvml = nv.nvmlDeviceGetHandleByIndex(phys)
             self.mx.append(int(nv.nvmlDeviceGetMaxClockInfo(self.nvml, nv.NVML_CLOCK_SM)))
+            self.power_limit = nv.nvmlDeviceGetPowerManagementLimit(self.nvml) / 1000.0
             self.thread = threading.Thread(target=self._nvml_loop, daemon=True); self.thread.start()
             return
         except Exception:
             self.nvml = None
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), "--query-gpu=clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,"
-                                          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap",
+                                          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit",
                                           "--format=csv,noheader,nounits", "-lms", "50"], stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             self.thread = threading.Thread(target=self._smi_read, daemon=True); self.thread.start()
         except Exception:
@@ -206,6 +212,11 @@ class ClockSampler:
             for i in range(4):
                 if len(r) >= 6 and r[2 + i].lower().startswith("active"):
                     self.reasons.add(names[i])
+            if len(r) >= 7:
+                try:
+                    self.power_limit = float(r[6])
+                except ValueError:
+                    pass
 
     def stop(self):
         self.stop_flag.set()
@@ -214,7 +225,7 @@ class ClockSampler:
         if self.thread:
             self.thread.join(timeout=1.0)
         return {"sm_mhz": int(np.median(self.sm)) if self.sm else None, "sm_max_mhz": max(self.mx) if self.mx else None, "reasons": sorted(self.reasons),
-                "samples": len(self.sm), "source": "nvml" if self.nvml is not None else "nvidia-smi"}
+                "samples": len(self.sm), "source": "nvml" if self.nvml is not None else "nvidia-smi", "power_limit_w": self.power_limit}
 
 
 def load_rdo_jobs_module():
@@ -230,6 +241,44 @@ STAT_NAMES = ["cyc_interp", "cyc_me", "cyc_me_bi", "cyc_tx_chain", "cyc_coeff_bi
               "intra_samples", "ssd_sad_samples", "super_blocks"] + ["cyc_me_%d" % (8 << k) for k in range(5)] + ["cyc_tx_%d" % (4 << k) for k in range(6)] + \
              ["cyc_ip_%d" % (4 << k) for k in range(6)] + ["ph_" + n for n in ("other", "early_skip", "skip_merge_cand", "search", "inter_cand", "bipred", "intra_search", "intra_cand",
                                                                                "commit")] + ["me_stage_" + n for n in ("telescope", "candidates", "hexagon", "halfpel", "quarterpel")]
+
+
+DUMP_BYTES = 64 * 10 ** 6
+# leaf fields the bit writer reads only for some block modes (enc/write_bits.c write_block; SKIP 0, INTRA 1, INTER 2, BIPRED 3, MERGE 4)
+LEAF_FIELD_MODES = {"intra_mode": (1,), "pb_part": (2, 3), "skip_idx": (0, 4)}
+
+
+def dump_outputs(path, frames):
+    """what tb_rdo_encode_frames returns for the frames of one step (reconstruction, block state, leaf lists, coefficients), as <name>.npy (float32; float64 where an integer needs more than 24 bits).
+    The dump stays under DUMP_BYTES: arrays smaller than an even share of what is left are written whole, each larger one as a fixed seeded
+    sample of its elements (sorted flat indices)."""
+    arrays = {}
+    for p, name in enumerate(("y", "u", "v")):
+        arrays["rec_" + name] = np.concatenate([hf.rec[p].reshape(-1) for hf in frames])
+    for n in frames[0].blk.dtype.names:
+        if n != "pad":
+            arrays["blk_" + n] = np.concatenate([hf.blk[n].reshape(-1) for hf in frames])
+    arrays["leaf_count"] = np.concatenate([hf.leaf_count for hf in frames])
+    valid = [hf.leaves[s, :hf.leaf_count[s]] for hf in frames for s in range(hf.job.nsb)]  # entries past leaf_count are not written
+    leaves = np.concatenate(valid)
+    arrays["sb_cost"] = np.array([int(v["cost"].astype(np.int64).sum()) for v in valid], np.int64)
+    # the quantised coefficients the bit writer codes, leaf by leaf (only the entries the leaves reference are written)
+    RJ = load_rdo_jobs_module()
+    arrays["coeffs"] = np.concatenate([np.zeros(0, np.int16)] + [RJ.leaf_coeffs(leaf, hf.coeffs[s]) for hf in frames for s in range(hf.job.nsb) for leaf in hf.leaves[s, :hf.leaf_count[s]]])
+    for n in leaves.dtype.names:
+        v = leaves[n]
+        if n in LEAF_FIELD_MODES:  # written from whichever candidate state the block's warp held last: -1 where the block's mode does not read it
+            v = np.where(np.isin(leaves["mode"], LEAF_FIELD_MODES[n]), v.astype(np.int16), -1)
+        arrays["leaf_" + n] = v.reshape(-1)
+    arrays = {k: (a.astype(np.float64) if a.size and np.abs(a.astype(np.int64)).max() >= 1 << 24 else a.astype(np.float32)) for k, a in arrays.items()}
+    os.makedirs(path, exist_ok=True)
+    left = DUMP_BYTES - 256 * len(arrays)  # .npy headers
+    for i, (k, a) in enumerate(sorted(arrays.items(), key=lambda kv: kv[1].nbytes)):
+        share = left // (len(arrays) - i)
+        if a.nbytes > share:
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, share // a.itemsize, replace=False))]
+        np.save(os.path.join(path, k + ".npy"), a)
+        left -= a.nbytes
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -379,6 +428,8 @@ def run_gpu(args, cfg):
         coll_ms = c0.elapsed_time(c1) + c2.elapsed_time(c3)
     clocks = sampler.stop()
     launches = int(L.tb_rdo_launch_count()) - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, hosts[nfr * (Ke - 1):nfr * Ke])
 
     # ---- parity: every frame of the end-to-end launch against the reference's decisions
     par = {"rec": 0, "blk": 0, "sb_cost": 0}
@@ -400,27 +451,23 @@ def run_gpu(args, cfg):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     value = world * K * gop_pixels / (ms * 1e-3) / 1e6
     e2e_value = world * Ke * gop_pixels / (ems * 1e-3) / 1e6
     alg_samples = st["search_samples"] + st["prediction_samples"] + st["txfm_samples"] + st["intra_samples"] + st["ssd_sad_samples"]
     alg_bytes = alg_samples * cfg.ESZ
     achieved = alg_bytes / (ms * 1e-3) / 1e9
     busy = 1.0 - st["cyc_idle"] / max(1, st["cyc_total"])
-    tr = None
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))[cfg.name]["rdo_batch_kernel"]
-    except Exception:
-        pass
     S = "uint8_t" if cfg.ESZ == 1 else "uint16_t"
     line = {
         "metric": cfg.metric(), "value": round(value, 4), "unit": "Mpixel/s", "n_gpus": world, "steps": K, "warmup": Wm, "ms_per_step": round(ms / K, 2),
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u8" if cfg.ESZ == 1 else "u16", "data": "synthetic",
         "config": {"workload": cfg.workload(), "frames_per_step": nfr, "steps_in_one_launch": K, "ctas": grid,
                    "parallelism": ("GOP-per-GPU x%d; rank 0 scatters the raw source frames over NCCL and gathers one int32 per super block from every rank (stand-in payload of the size of the RD costs; the decisions themselves are downloaded to each rank's host)" % world) if world > 1 else "1 GPU, no collective",
-                   "l2_policy": "per-launch inputs+outputs %.0f MB > 126 MB L2" % ((h2d + d2h) * K / 1e6)},
+                   "l2_policy": "per-launch inputs+outputs %.0f MB, L2 %.0f MB" % ((h2d + d2h) * K / 1e6, torch.cuda.get_device_properties(local).L2_cache_size / 1e6)},
         "e2e": {"value": round(e2e_value, 4), "unit": "Mpixel/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h), "ms_per_step": round(ems / Ke, 2), "steps": Ke},
         "gpu_launches": launches,
+        "gpu": {"name": torch.cuda.get_device_name(local), "power_limit_w": clocks.pop("power_limit_w")},
         "clocks": clocks,
         "parity": {"frames_checked": nchk, "rec_equal": par["rec"], "block_state_equal": par["blk"], "sb_cost_equal": par["sb_cost"], "ok": parity_ok,
                    "checker": "reference (process_block of the compiled reference encoder, captured with the jobs)"},
@@ -428,15 +475,10 @@ def run_gpu(args, cfg):
                      # contract fields: ALGORITHMIC bytes (SURVEY.md §8d per-unit figures x the units the data-dependent loop actually executed, counted by the kernel)
                      # / launch time vs the measured HBM peak.  The kernel is NOT HBM-bound: it is a dependency chain (serial block decisions inside a super
                      # block, wavefront between super blocks); what bounds it is single-warp latency, see `binding`
-                     "bound": "hbm", "achieved": round(achieved, 2), "peak": peak, "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)",
+                     "bound": "hbm", "achieved": round(achieved, 2), "peak": peak, "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, 3.35 TB/s HBM3",
                      "unit": "GB/s", "frac": round(achieved / peak, 5),
-                     # DRAM bytes of this launch, scaled per super block from the committed ncu capture of the same kernel on a smaller batch (profiles/ncu_traffic.json)
-                     "traffic": int(tr["dram_bytes_total"] / tr["super_blocks"] * st["super_blocks"]) if tr and tr.get("super_blocks") else None,
-                     "traffic_source": tr.get("capture") if tr else None,
-                     "binding": "instruction delivery (ncu: ~19 stalled warps per issued instruction wait for instructions; issue slots 4 % busy; DRAM 0.1 %, L2 2 % of peak): "
-                                "a serial decision chain per super block run by one 8-warp CTA whose code streams from L2",
+                     "binding": "a serial decision chain per super block run by one 8-warp CTA whose code streams from L2",
                      "cta_busy_frac": round(busy, 4), "algorithmic_bytes": int(alg_bytes), "ms_per_launch": round(ms, 2), "share_of_step": 1.0,
-                     "ncu": {k: tr[k] for k in tr if k.endswith("_pct") or k.startswith("stalled_")} if tr else None,
                      "work": {k: st[k] for k in STAT_NAMES[11:23]},
                      "cycles_share": {k[4:]: round(st[k] / max(1, st["cyc_total"]), 4) for k in STAT_NAMES[:10] + STAT_NAMES[23:40]},
                      "phase_share_of_a_super_block": {k[3:]: round(st[k] / max(1, sum(st[n] for n in STAT_NAMES[40:49])), 4) for k in STAT_NAMES[40:49]},
@@ -621,6 +663,7 @@ def main():
     ap.add_argument("--cache", default=os.environ.get("THOR_B200_CACHE", "/tmp/thor_b200_bench"))
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--cpu-fresh", action="store_true", help="cpu_baseline: measure again even if a recent measurement of this box exists in the cache")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the decisions of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     cfg = Cfg(args.config, tuple(int(v) for v in args.size.split("x")) if args.size else None, args.frames or None)
     os.makedirs(args.cache, exist_ok=True)

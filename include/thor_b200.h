@@ -1,4 +1,4 @@
-/* thor_b200.h — C ABI of libthor_b200.so, the B200 (sm_100a) implementation of the cisco/thor per-block hot path.
+/* thor_b200.h — C ABI of libthor_b200.so, the H100 (sm_90a) implementation of the cisco/thor per-block hot path.
  *
  * Two faces (DESIGN.md §2):
  *

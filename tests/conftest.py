@@ -7,7 +7,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: -m gpu)")
     config.addinivalue_line("markers", "ref: needs oracle/_ref (the compiled reference); skipped when absent")
 
 

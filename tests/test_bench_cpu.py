@@ -1,5 +1,5 @@
 """bench.py's CPU arm (`--impl reference`) end to end on a small clip: the reference encoders start, the observing shim publishes progress, one JSON line with the contract's
-keys comes out.  (The GPU arm needs a B200; its workload capture and job parsing are covered by tests/test_rdo_jobs.py.)"""
+keys comes out.  (The GPU arm needs a GPU; its workload capture and job parsing are covered by tests/test_rdo_jobs.py.)"""
 import json
 import os
 import subprocess

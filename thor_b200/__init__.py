@@ -1,4 +1,4 @@
-"""thor_b200 — ctypes face of libthor_b200.so (the sm_100a CUDA implementation of the Thor per-block hot path).
+"""thor_b200 — ctypes face of libthor_b200.so (the sm_90a CUDA implementation of the Thor per-block hot path).
 
 This package is plumbing only: it loads the in-tree shared library built by thor_b200/build.py, declares the C ABI of
 include/thor_b200.h, and offers numpy record dtypes for the work-item structs.  There is no CPU implementation here;

@@ -1,4 +1,4 @@
-"""Build libthor_b200.so (sm_100a only) in-tree with nvcc.  Used by __graft_entry__.build() and the tests."""
+"""Build libthor_b200.so (sm_90a only) in-tree with nvcc.  Used by __graft_entry__.build() and the tests."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libthor_b200.so")
 SOURCES = ["tb_api.cu", "tb_rdo.cu"]
 DEPS = sorted(f for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh", ".h"))) + [os.path.join("..", "..", "include", "thor_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "--std=c++17", "-shared", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "--std=c++17", "-shared", "-Xcompiler", "-fPIC",
               "-Xptxas", "-v", "--use_fast_math=false"]
 
 

@@ -25,7 +25,7 @@ struct Ctx {
   static constexpr int NSLOT = 8;  // 0-3 operand windows, 4-6 compact copies, 7 filter flags
   void *slot[NSLOT] = {nullptr};
   size_t cap[NSLOT] = {0};
-  int sm_count = 148;
+  int sm_count = 132;  // H100 SXM; replaced by the device's count in ensure_ctx()
   unsigned long long *me_stats = nullptr;
 };
 Ctx g;

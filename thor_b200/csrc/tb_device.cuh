@@ -1,4 +1,4 @@
-// tb_device.cuh — warp-level device routines of the Thor hot path for sm_100a.
+// tb_device.cuh — warp-level device routines of the Thor hot path for sm_90a (H100).
 //
 // Execution model: ONE WARP PER WORK ITEM (coding / prediction / transform block, or one motion search).  Small
 // blocks are packed several-probes-per-warp inside the routines so all 32 lanes stay busy.  Samples are handled as
@@ -22,7 +22,7 @@
 #define TB_ME_QUAD_SIZE16 1  // also the 8x8 partitions of 16x16 coding blocks (wide-SAD candidate stage)
 #endif
 #ifndef TB_QUAD_HALFPEL_PLANES
-#define TB_QUAD_HALFPEL_PLANES 0  // group form of the half-pel planes inside quad_motion_estimate: bit-exact, measured slower (cb8 class 6.2 vs 5.3 ms)
+#define TB_QUAD_HALFPEL_PLANES 0  // group form of the half-pel planes inside quad_motion_estimate: bit-exact, slower than the per-warp form
 #endif
 #ifndef TB_SAD_V4
 #define TB_SAD_V4 1  // 128-bit loads for block rows of >= 16 bytes
@@ -32,14 +32,14 @@
 #endif
 #ifndef TB_SUBPEL_SHARED
 // 1: sub-pel stages through subpel_stage_sads_shared (horizontally filtered rows shared between the eight probes via shared
-// memory).  Bit-exact, but measured SLOWER on B200 (sub-pel share of the 1080p batch 9.4 ms vs 6.8 ms): per 16x16 tile it
+// memory).  Bit-exact, but slower than the register form: per 16x16 tile it
 // executes only ~1.2x fewer instructions than the per-probe register form (22 filtered rows per 16 output rows, five planes)
 // and adds two shared-memory round trips per tile to every warp's dependency chain; 22 KB of shared memory per CTA also
-// shrinks L1.  Kept as a measured alternative.
+// shrinks L1.  Kept as an alternative.
 #define TB_SUBPEL_SHARED 0
 #endif
 #ifndef TB_TX_MINBLOCKS
-#define TB_TX_MINBLOCKS 6  // __launch_bounds__(128, N) of the transform-chain kernel (measured: 4: 5.84 ms, 5: 5.37, 6: 5.12)
+#define TB_TX_MINBLOCKS 6  // __launch_bounds__(128, N) of the transform-chain kernel: registers/thread <= 65536 / (128 N)
 #endif
 #ifndef TB_ME_MINBLOCKS
 #define TB_ME_MINBLOCKS 6  // __launch_bounds__(128, N) of the motion-search kernel: registers/thread <= 65536 / (128 N)
@@ -113,7 +113,7 @@ template <class S> __device__ __forceinline__ int word_px(uint32_t w, int i) {
 // Lanes sub..sub+nl-1 of a group share the block; returns this lane's partial sum.
 // ---------------------------------------------------------------------------------------------------------------
 // Rows of >= 16 bytes with 128-bit loads: one aligned LDG.128 per 16 reference bytes (+1 per row) and one per 16 original
-// bytes instead of eight 32-bit loads — the search is bound by L1 wavefronts (59 % of the l1tex data-pipe peak in ncu), so
+// bytes instead of eight 32-bit loads — the search is designed for L1 wavefronts as its bound, so
 // request count matters more than bytes.  J = word offset of the row inside its first 16-byte chunk (uniform per lane group:
 // all pitches are multiples of 16 bytes), sh = remaining byte offset in bits.
 template <class S, int J>
@@ -1216,8 +1216,7 @@ __device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_fu
 // ---------------------------------------------------------------------------------------------------------------
 // a5 for small blocks: FOUR searches per warp, eight lanes each.  A search over a block of <= 64 samples spends most of its
 // instructions in stages that can use only 3-8 lanes (candidate list, hexagon rounds, the eight sub-pel probes) and in per-stage
-// scalar work (clipping, pricing, winner selection); sharing the warp between four searches issues that work once for four
-// (profiles/r1_ncu_summary.md section E: 4.2 k warp instructions per search, a third of the stalls are instruction fetches).
+// scalar work (clipping, pricing, winner selection); sharing the warp between four searches issues that work once for four.
 // Every lane of a group carries its search's state; all collectives use the group's 8-lane mask, so groups diverge freely.
 // Same stages, visiting order and tie rules as warp_motion_estimate (8-bit samples, speed 0).
 // ---------------------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// tb_kernels.cuh — __global__ kernels of libthor_b200 (sm_100a).  Block-level kernels: one warp per work item,
+// tb_kernels.cuh — __global__ kernels of libthor_b200 (sm_90a).  Block-level kernels: one warp per work item,
 // grid-stride over the item array.  Frame-level kernels: one thread per sample / edge, laid out so that lanes walk
 // along rows (coalesced 128-byte requests).  See DESIGN.md §4 for the roofline of each kernel.
 #pragma once
@@ -262,7 +262,7 @@ template <class S> __global__ void __launch_bounds__(CTA_THREADS) combine_batch_
 // Four consecutive items per warp and step.  85 % of the predictions of an encode are blocks of <= 64 samples (4x4 ... 8x8 luma,
 // 2x2 ... 8x8 chroma) whose cost is one dependent chain item -> samples -> store: when all four are that small, each gets a group
 // of eight lanes and the four chains overlap; otherwise the warp takes them one after the other.  (Eight groups of four lanes for
-// blocks of <= 16 samples were measured slower: 96 registers instead of 72, 1.81 ms instead of 1.57 ms for the 1080p batch.)
+// blocks of <= 16 samples were slower: 96 registers instead of 72.)
 template <class S> __global__ void __launch_bounds__(CTA_THREADS) interp_batch_kernel(const tb_interp_item_t *items, int n, int bitdepth, int bip) {
   const int lane = lane_id(), grp = lane >> 3;
   for (int base = global_warp() * 4; base < n; base += total_warps() * 4) {

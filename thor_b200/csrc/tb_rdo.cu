@@ -292,8 +292,7 @@ template <class S> struct DevBackend {
   }
   // <= 12 chains of 4x4 / 8x8 transform blocks (residual -> DCT -> quantiser -> dequantiser -> inverse DCT -> reconstruction, the arithmetic of
   // common/transform.c:245-308, 411-494, enc/encode_block.c:84-171, common/common_block.c:45-83), all of them together on the warp.  Written as LOOPS over
-  // (chain, element) work items dealt to the lanes: the RD loop is bound by instruction fetch (ncu: 19 stalled warps per issued instruction wait for
-  // instructions), so a few hundred instructions that stay in the instruction cache beat the unrolled one-thread-per-chain forms (5.6 k instructions
+  // (chain, element) work items dealt to the lanes: the RD loop is bound by instruction fetch, so a few hundred instructions that stay in the instruction cache beat the unrolled one-thread-per-chain forms (5.6 k instructions
   // streamed from L2 per call).  Tiles of 64 int16 per chain in the warp's scratch; the quantiser's level-mode walk is sequential: one lane per chain.
   __device__ __noinline__ void tx_multi(const tbr::TxJob<S> *jobs, int n, int *bit) const {
     PROF2(PF_TX, ST_TX_SZ + ilog2(jobs[0].size) - 2);
@@ -637,7 +636,7 @@ __global__ void __launch_bounds__(32 * RDO_WARPS, TB_RDO_CTAS_PER_SM)
       sel = cta.sel;
       if (sel == 0x7fffffff) {  // nothing ready: finished, failed, or wait for the running super blocks
         if (threadIdx.x == 0) {
-          // ONE thread polls ONE word (the event counter) at a low rate: a super block takes ~100 ms, and every CTA of the grid scanning the row
+          // ONE thread polls ONE word (the event counter) at a low rate: a super block takes many polling intervals, and every CTA of the grid scanning the row
           // table in a tight loop turns its few cache lines into a hot spot of one L2 slice that slows the working CTAs down
           int f = 0;
           const int ev0 = cta.x_idx[1];

@@ -28,7 +28,7 @@
 #define TBR_NO_OVERLAP 0  // 1: every block through the serial form of mode_decision_rdo (A/B)
 #endif
 // TBR_NI: the functions of the control flow exist ONCE in the device code (no inlining at their many call sites): the RD loop is one kernel whose warps run
-// different parts of it at the same time, and an all-inlined build (2.5 MB of SASS) lives on instruction fetches from L2
+// different parts of it at the same time, and an all-inlined build (several MB of SASS) lives on instruction fetches from L2
 #ifdef __CUDACC__
 #define TBR_NI __noinline__
 #else

@@ -35,6 +35,22 @@ RDO_LEAF = np.dtype([("xpos", "u2"), ("ypos", "u2"), ("size", "u1"), ("mode", "u
 assert RDO_BLK.itemsize == 20 and RDO_LEAF.itemsize == 64
 
 
+def coeff_count(size, tb_split):
+    """tb_rdo_coeff_count (include/thor_b200.h): int16 coefficients stored for one plane of a coded block"""
+    t = size // 2 if tb_split else size
+    q = min(t, 16)
+    return (4 if tb_split else 1) * q * q
+
+
+def leaf_coeffs(leaf, coeffs):
+    """the quantised coefficients of one leaf (Y, then U, then V) inside its super block's coefficient area; empty when it has none"""
+    ofs, size, split = int(leaf["coeff_ofs"]), int(leaf["size"]), int(leaf["tb_split"])
+    if ofs < 0:
+        return coeffs[:0]
+    sc = size >> 1
+    return coeffs[ofs:ofs + coeff_count(size, split) + 2 * coeff_count(sc, int(split and sc > 4))]
+
+
 class Job:
     """one frame_NNN.job: .hdr (RdoFrame with NULL pointers), .frame_num, .nsb, .orig[3], .refs[r][3] (whole padded planes), and the reference's
     results .rec[3], .blk, .sb_cost"""

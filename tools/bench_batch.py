@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — Thor per-block hot path on B200: encode-side hot-path throughput in Mpixel/s.
+"""bench.py — Thor per-block hot path on one GPU: encode-side hot-path throughput in Mpixel/s.
 
 ONE STEP = one pass of the hot path over one inter frame's worth of work, in the quantities the reference's RD loop
 generates for the chosen encoder configuration when no early termination fires (enc/encode_block.c:1835-2120, 2401-2565):
@@ -651,12 +651,12 @@ def run_gpu(args, cfg):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_source = "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_source = "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, 3.35 TB/s HBM3"
 
     def ncu_of(kernel):
-        """DRAM bytes per launch + the binding ncu roofs of this kernel from the committed `ncu --set full` capture of the same workload
-        (profiles/ncu_traffic.json, written from the round's capture; keyed by config and kernel)"""
+        """DRAM bytes per launch + the binding ncu roofs of this kernel from an `ncu --set full` capture of the same workload
+        (profiles/ncu_traffic.json, keyed by config and kernel; None when there is no capture)"""
         try:
             tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))[cfg.name][kernel]
             return tr
@@ -668,10 +668,9 @@ def run_gpu(args, cfg):
         traffic = int(tr["dram_bytes_read"] + tr["dram_bytes_write"]) if tr and tr.get("items") == extra.get("items") else None
         achieved = alg_bytes / (k_ms * 1e-3) / 1e9
         r = {"kernel": label,
-             # `achieved`/`frac` follow the bench contract: ALGORITHMIC bytes (SURVEY.md §8d) / launch time vs the measured HBM copy peak.  These bytes
-             # are an L1/L2 stream of cache-resident frames, NOT HBM traffic: the kernel is bound by issue slots and L1 wavefronts (ncu), so the
-             # binding roofs and the real DRAM rate are reported beside it.
-             "bound": "issue+l1 (per ncu; frames are L2-resident, DRAM is not the roof)", "achieved": round(achieved, 1), "peak": peak, "peak_source": peak_source, "unit": "GB/s",
+             # `achieved`/`frac` follow the bench contract: ALGORITHMIC bytes (SURVEY.md §8d) / launch time vs the HBM peak.  These bytes are
+             # mostly served from L1/L2, not HBM, so an ncu capture's real DRAM rate is reported beside it when one is given.
+             "bound": "issue+l1 (by design; not profiled on this GPU)", "achieved": round(achieved, 1), "peak": peak, "peak_source": peak_source, "unit": "GB/s",
              "frac": round(achieved / peak, 4), "l1_stream_gbs": round(achieved, 1), "traffic": traffic,
              "dram_gbs": round(traffic / (k_ms * 1e-3) / 1e9, 1) if traffic else None, "dram_frac": round(traffic / (k_ms * 1e-3) / 1e9 / peak, 4) if traffic else None,
              "ncu": {k: tr[k] for k in tr if k.endswith("_pct")} if tr else None,
@@ -692,7 +691,7 @@ def run_gpu(args, cfg):
         "config": {"workload": workload,
                    "parallelism": ("frame-per-GPU x%d; per step rank 0 scatters the raw frames and gathers the search decisions over NCCL" % world) if world > 1 else
                                   "frame-per-GPU x1, no collective",
-                   "l2_policy": "per-step inputs+outputs %.0f MB > 126 MB L2" % (resident_bytes / 1e6)},
+                   "l2_policy": "per-step inputs+outputs %.0f MB, L2 %.0f MB" % (resident_bytes / 1e6, torch.cuda.get_device_properties(local).L2_cache_size / 1e6)},
         "e2e": {"value": round(e2e_value, 3), "unit": "Mpixel/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h), "ms_per_step": round(ems / args.steps, 3)},
         "gpu_launches": launches,
         "clocks": clocks,

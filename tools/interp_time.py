@@ -1,4 +1,4 @@
-"""Time interp_batch_kernel and intra_batch_kernel on the bench workload (B200 only)."""
+"""Time interp_batch_kernel and intra_batch_kernel on the bench workload (needs a GPU)."""
 import ctypes as C, os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Time me_batch_kernel per coding-block size class of the bench workload (B200 only; writes a small table to stdout)."""
+"""Time me_batch_kernel per coding-block size class of the bench workload (needs a GPU; writes a small table to stdout)."""
 import ctypes as C, json, os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Instruction counts of the device functions inside rdo_batch_kernel (nvdisasm of the sm_100a cubin of tb_rdo.cu), as markdown: the RD loop is bound by instruction
-delivery (profiles/r2_ncu_rdo_summary.md), so the size of what each phase streams from L2 is the quantity to watch.  Usage: python tools/rdo_code_size.py [out.md]"""
+"""Instruction counts of the device functions inside rdo_batch_kernel (nvdisasm of the sm_90a cubin of tb_rdo.cu), as markdown: the RD loop is bound by instruction
+delivery, so the size of what each phase streams from L2 is the quantity to watch.  Usage: python tools/rdo_code_size.py [out.md]"""
 import collections
 import os
 import re
@@ -37,8 +37,8 @@ def main():
         dem = re.sub(r"\(.*", "", dem)
         dem = re.sub(r"Rdo<unsigned (char|short), DevBackend<unsigned (char|short)> >", "Rdo", dem)
         rows[kern].append((n, dem))
-    lines = ["# Device functions of rdo_batch_kernel by size (`nvdisasm` of tb_rdo.cu's sm_100a cubin; SASS instructions, 16 bytes each)", "",
-             "First correct build of the round: everything inlined, 157 k instructions (2.5 MB) for the 8-bit kernel.  Now every function of the control flow and of the backend exists",
+    lines = ["# Device functions of rdo_batch_kernel by size (`nvdisasm` of tb_rdo.cu's sm_90a cubin; SASS instructions, 16 bytes each)", "",
+             "An all-inlined build is several MB of SASS.  Every function of the control flow and of the backend exists",
              "once per kernel (`__noinline__`), the per-sample loops are rolled, the small transform chains are loops.", ""]
     for kern, r in rows.items():
         r.sort(reverse=True)

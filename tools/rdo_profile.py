@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """One launch of rdo_batch_kernel over the inter frames of a captured clip, for ncu / compute-sanitizer:
-  ncu --set full --import-source on --clock-control none -k regex:rdo_batch -c 1 -o gpurun_out/rdo python tools/rdo_profile.py --size 640x384
+  ncu --set full --import-source on --clock-control none -k regex:rdo_batch -c 1 -o rdo python tools/rdo_profile.py --size 640x384
 Prints the kernel's own counters (cycles per primitive class, work executed)."""
 import argparse
 import ctypes as C

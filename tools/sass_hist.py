@@ -9,7 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "thor_b200", "libthor_b200.so")
-INTEREST = ["VABSDIFF4", "IDP.4A", "IDP.2A", "IDP", "IMAD", "LDG", "LDS", "STS", "STG", "SHFL", "BAR", "UTMALDG", "UBLKCP", "UTCMMA", "LDTM", "SYNCS", "HMMA", "IMMA", "DMUL", "DADD", "DFMA",
+INTEREST = ["VABSDIFF4", "IDP.4A", "IDP.2A", "IDP", "IMAD", "LDG", "LDS", "STS", "STG", "SHFL", "BAR", "UTMALDG", "UBLKCP", "SYNCS", "HMMA", "IMMA", "DMUL", "DADD", "DFMA",
             "ATOM", "RED", "LDL", "STL", "I2IP", "VOTE", "MATCH"]
 
 
@@ -38,10 +38,10 @@ def main():
                     break
         rows.append((total, k, agg))
     rows.sort(reverse=True)
-    cols = ["VABSDIFF4", "IDP.4A", "IDP.2A", "IMAD", "LDG", "LDS", "STS", "SHFL", "BAR", "LDL", "STL", "DMUL", "DADD", "UTMALDG", "UBLKCP", "UTCMMA", "IMMA", "HMMA"]
-    lines = ["# SASS opcode histogram per kernel (`cuobjdump -sass thor_b200/libthor_b200.so`, sm_100a)", "",
+    cols = ["VABSDIFF4", "IDP.4A", "IDP.2A", "IMAD", "LDG", "LDS", "STS", "SHFL", "BAR", "LDL", "STL", "DMUL", "DADD", "UTMALDG", "UBLKCP", "IMMA", "HMMA"]
+    lines = ["# SASS opcode histogram per kernel (`cuobjdump -sass thor_b200/libthor_b200.so`, sm_90a)", "",
              "Static instruction counts (not executed counts).  LDL/STL = local-memory (spill or per-thread array) accesses; UTMALDG/UBLKCP = TMA bulk copies;",
-             "UTCMMA = tcgen05 MMA; IMMA/HMMA = mma.sync tensor-core ops.", "",
+             "IMMA/HMMA = mma.sync tensor-core ops.", "",
              "| kernel | SASS instrs | " + " | ".join(cols) + " |", "|---|---|" + "---|" * len(cols)]
     for total, k, agg in rows:
         if total < 50:

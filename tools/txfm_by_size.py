@@ -1,4 +1,4 @@
-"""Time txfm_chain_kernel per transform size of the bench workload (B200 only)."""
+"""Time txfm_chain_kernel per transform size of the bench workload (needs a GPU)."""
 import ctypes as C, os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
