@@ -32,13 +32,13 @@ def _compile(src, obj, flags):
     return r.returncode, " ".join(cmd) + "\n" + r.stdout + r.stderr
 
 
-def build(force=False, verbose=False, defines=(), out=None):
+def build(force=False, verbose=False):
     """one object per translation unit (compiled in parallel, kept under thor_b200/build/ and reused while its sources are older), then one link"""
-    if not force and not stale() and out is None:
+    if not force and not stale():
         return LIB
     from concurrent.futures import ThreadPoolExecutor
-    flags = [f for f in NVCC_FLAGS if not f.startswith("--use_fast_math") and f != "-shared"] + ["-D" + d for d in defines]
-    objdir = os.path.join(HERE, "build", "default" if out is None else os.path.basename(out))
+    flags = [f for f in NVCC_FLAGS if not f.startswith("--use_fast_math") and f != "-shared"]
+    objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
     newest = max(os.path.getmtime(os.path.join(CSRC, d)) for d in DEPS)
     jobs = []
@@ -53,17 +53,17 @@ def build(force=False, verbose=False, defines=(), out=None):
             if rc != 0:
                 sys.stderr.write(text)
                 raise RuntimeError("nvcc failed building libthor_b200.so")
-    cmd = [nvcc(), "-shared", "-o", out or LIB] + [os.path.join(objdir, s.replace(".cu", ".o")) for s in SOURCES]
+    cmd = [nvcc(), "-shared", "-o", LIB] + [os.path.join(objdir, s.replace(".cu", ".o")) for s in SOURCES]
     r = subprocess.run(cmd, capture_output=True, text=True)
     log += " ".join(cmd) + "\n" + r.stdout + r.stderr
-    with open(os.path.join(HERE, "build.log") if out is None else out + ".log", "w") as f:  # A/B builds log next to their output (ab_libs/)
+    with open(os.path.join(HERE, "build.log"), "w") as f:
         f.write(log)
     if r.returncode != 0:
         sys.stderr.write(log)
         raise RuntimeError("nvcc failed linking libthor_b200.so")
     if verbose:
         print(log)
-    return out or LIB
+    return LIB
 
 
 if __name__ == "__main__":
