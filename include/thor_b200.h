@@ -312,6 +312,16 @@ int tb_rdo_batch_grid(const tb_rdo_batch_t *b);                                 
                             [40..48]: wall cycles of a CTA by decision phase (other, early skip, skip/merge candidates, searches, inter candidates, bipred, intra search,
                             intra candidates, commit); [49..53]: cycles of the searches of blocks <= 16 by stage (telescope, candidates, hexagon, half-pel, quarter-pel) */
 int tb_rdo_batch_stats(const tb_rdo_batch_t *b, uint64_t *out, int n);
+/* timeline of the last synchronised launch: one entry per super block, in the order they finished.  Times are the GPU's global nanosecond
+ * timer (%globaltimer), comparable between SMs.  A super block starts after the super blocks it depends on have ended. */
+typedef struct {
+  int32_t frame, row, col; /* slot of the batch, super-block row and column */
+  int32_t cta;             /* blockIdx.x of the CTA that decided it */
+  uint64_t t_start, t_end; /* ns */
+} tb_rdo_sb_trace_t;
+/* copies min(n, super blocks of the last launch) entries to out and returns how many (TB_ERR_CUDA if the copy fails);
+ * out == NULL: returns the super blocks of the last launch */
+int tb_rdo_batch_trace(const tb_rdo_batch_t *b, tb_rdo_sb_trace_t *out, int n);
 void tb_rdo_batch_destroy(tb_rdo_batch_t *b);
 const char *tb_rdo_last_error(void);
 uint64_t tb_rdo_launch_count(void);

@@ -67,7 +67,8 @@ struct RdoCta {
   uint32_t x_sad[TB_RDO_MAX_REF];
   alignas(16) int x_buf[32];
   int x_queue[4];
-  int sel;
+  unsigned long long sel;   // claim of the scheduler: (remaining path << 32) | (0xffffffff - row index), max over the CTA
+  unsigned long long t_sb;  // %globaltimer when the current super block started
 };
 // per-warp scratch
 template <class S> struct RdoShared {
@@ -580,19 +581,30 @@ constexpr int RDO_WARPS = 8;  // warps per CTA: 8 x 32 threads x 255 registers =
 constexpr int RDO_CTAS_PER_SM = 1;
 
 // One row of super blocks of one frame of the batch.  Rows are the unit a CTA claims; super blocks inside a row are sequential.
-struct RowDesc { int frame, row, nsbx, pad; };
+// path = nsbx + 2 (nsby - 1 - row): super blocks on the longest dependency chain from the row's first super block to the end of its frame.
+struct RowDesc { int frame, row, nsbx, path; };
 // scheduler words behind the per-row arrays
 enum { CTL_REMAINING = 0, CTL_ERROR = 1, CTL_EVENT = 2 /* bumped after every finished super block */, CTL_N = 4 };
 
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
 // Persistent CTAs draw READY super blocks from the rows of every frame of the batch (dataflow scheduling): row r of a frame may process
 // super block c when row r-1 has published min(c+2, nsbx) super blocks (left, up-left, up, up-right neighbours: get_mv_pred / intra
-// prediction / block contexts read nothing else); frames are independent of each other.  A CTA claims a ready row (lowest index first:
-// the top rows of the earliest frames unblock the most work), processes super blocks while the next one is ready, then releases the row,
-// so a CTA never holds an SM while it waits for a neighbour: a row migrates between CTAs at super-block boundaries (all per-super-block
-// state is re-initialised by process_sb; data of other super blocks is read through L2, see TB_LDF above).
+// prediction / block contexts read nothing else); frames are independent of each other.  A CTA claims the ready row with the longest
+// remaining dependency chain, path - progress (ties: the lower row index): the launch ends when the last frame's chain ends, so the rows
+// that chain runs through go first, and a frame's lower rows are not left waiting behind the last rows of other frames.  It processes ONE
+// super block, releases the row and chooses again (replayed on measured H100 timelines, re-choosing after every super block ends the
+// bench launch about 6 % sooner than staying in the row while it is ready), so a CTA never holds an SM while it waits for a neighbour: a
+// row migrates between CTAs at super-block boundaries (all per-super-block state is re-initialised by process_sb; data of other super
+// blocks is read through L2, see TB_LDF above).  Every finished super block is recorded in trace[] in completion order (tb_rdo_batch_trace).
 template <class S>
 __global__ void __launch_bounds__(32 * RDO_WARPS, RDO_CTAS_PER_SM)
-    rdo_batch_kernel(const FrameCtx<S> *ctxs, const RowDesc *rows, int nrows, Work<S> *works, int *prog, int *claimed, int *ctl, unsigned long long *prof_out) {
+    rdo_batch_kernel(const FrameCtx<S> *ctxs, const RowDesc *rows, int nrows, Work<S> *works, int *prog, int *claimed, int *ctl, unsigned long long *prof_out,
+                     tb_rdo_sb_trace_t *trace) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   RdoCta &cta = *(RdoCta *)smem_raw;
   FrameCtx<S> &fctx = *(FrameCtx<S> *)(smem_raw + ((sizeof(RdoCta) + 15) & ~(size_t)15));
@@ -615,19 +627,22 @@ __global__ void __launch_bounds__(32 * RDO_WARPS, RDO_CTAS_PER_SM)
     int sel;
     {
       Prof pw(sh.prof, PF_WAIT);
-      if (threadIdx.x == 0) { cta.sel = 0x7fffffff; cta.x_idx[1] = vctl[CTL_EVENT]; }  // the event count BEFORE the scan: progress made during the scan is not lost
+      if (threadIdx.x == 0) { cta.sel = 0; cta.x_idx[1] = vctl[CTL_EVENT]; }  // the event count BEFORE the scan: progress made during the scan is not lost
       __syncthreads();
-      int mine = 0x7fffffff;
+      unsigned long long mine = 0;  // (remaining path << 32) | (0xffffffff - row index): the larger, the more urgent; 0 = nothing ready
       for (int g = threadIdx.x; g < nrows; g += blockDim.x) {
         if (vclaimed[g]) continue;
         const RowDesc rd = rows[g];
         const int p = vprog[g];
-        if (p < rd.nsbx && (rd.row == 0 || vprog[g - 1] >= min(p + 2, rd.nsbx))) { mine = g; break; }
+        if (p < rd.nsbx && (rd.row == 0 || vprog[g - 1] >= min(p + 2, rd.nsbx))) {
+          const unsigned long long k = ((unsigned long long)(rd.path - p) << 32) | (0xffffffffu - (unsigned)g);
+          if (k > mine) mine = k;
+        }
       }
-      if (mine != 0x7fffffff) atomicMin(&cta.sel, mine);
+      if (mine) atomicMax(&cta.sel, mine);
       __syncthreads();
-      sel = cta.sel;
-      if (sel == 0x7fffffff) {  // nothing ready: finished, failed, or wait for the running super blocks
+      sel = cta.sel ? (int)(0xffffffffu - (unsigned)cta.sel) : -1;
+      if (sel < 0) {  // nothing ready: finished, failed, or wait for the running super blocks
         if (threadIdx.x == 0) {
           // ONE thread polls ONE word (the event counter) at a low rate: a super block takes many polling intervals, and every CTA of the grid scanning the row
           // table in a tight loop turns its few cache lines into a hot spot of one L2 slice that slows the working CTAs down
@@ -669,29 +684,28 @@ __global__ void __launch_bounds__(32 * RDO_WARPS, RDO_CTAS_PER_SM)
       cur_frame = rd.frame;
     }
     __syncthreads();
-    int sbx = cta.x_idx[0];
-    while (true) {
+    const int sbx = cta.x_idx[0];
+    {
       Rdo<S, DevBackend<S>> R(fctx, works[blockIdx.x * nw + wid], works[blockIdx.x * nw], be);
       if (lane == 0) sh.t_mark = clock64();
+      if (threadIdx.x == 0) cta.t_sb = globaltimer();
       R.process_sb(sbx, rd.row);
       be.mark(tbr::PH_OTHER);
       __threadfence();  // every writing thread orders its stores before the flag
       __syncthreads();
       if (threadIdx.x == 0) {
+        const unsigned long long t_end = globaltimer();  // before the progress is published: a dependent super block starts after it
         sh.prof[ST_SB] += 1;
         vprog[sel] = sbx + 1;
         atomicSub(&ctl[CTL_REMAINING], 1);
-        const int nx = sbx + 1;
-        const int cont = nx < rd.nsbx && (rd.row == 0 || vprog[sel - 1] >= min(nx + 2, rd.nsbx));
-        if (!cont) { __threadfence(); atomicExch(&claimed[sel], 0); }
         __threadfence();
-        atomicAdd(&ctl[CTL_EVENT], 1);
-        cta.x_flag[0] = cont;
+        atomicExch(&claimed[sel], 0);  // one super block per claim: the next claim re-chooses among all ready rows
+        __threadfence();
+        const int k = atomicAdd(&ctl[CTL_EVENT], 1);  // = super blocks finished before this one: its slot in the trace
+        tb_rdo_sb_trace_t e;
+        e.frame = cur_frame; e.row = rd.row; e.col = sbx; e.cta = blockIdx.x; e.t_start = cta.t_sb; e.t_end = t_end;
+        trace[k] = e;
       }
-      __syncthreads();
-      if (!cta.x_flag[0]) break;
-      __threadfence();
-      sbx++;
     }
     idle_since = clock64();
   }
@@ -741,6 +755,8 @@ struct tb_rdo_batch {
   int *ctl_host = nullptr;                       // pinned: ctl words read back after the launch
   void *works = nullptr;
   unsigned long long *prof = nullptr;
+  tb_rdo_sb_trace_t *trace = nullptr;            // one entry per super block of the last launch, in completion order
+  int nsb = 0, trace_cap = 0;
   unsigned long long stats[ST_END] = {};
   int sms = 0;
 };
@@ -807,7 +823,7 @@ int check_desc(const tb_rdo_frame_t *f) {
 }
 
 template <class S> int batch_launch(tb_rdo_batch *b, int n_active, cudaStream_t st) {
-  // rows of the active slots, frame-major: the lowest index is the most urgent row
+  // rows of the active slots, frame-major (the index breaks ties between rows of equal remaining path)
   int nrows = 0, nsb_total = 0;
   for (int s = 0; s < n_active; s++) { nrows += b->slots[s].nsby; nsb_total += b->slots[s].nsby * b->slots[s].nsbx; }
   if (nrows > b->nrows_cap) {
@@ -818,11 +834,19 @@ template <class S> int batch_launch(tb_rdo_batch *b, int n_active, cudaStream_t 
     CK(cudaMalloc((void **)&b->sched_dev, sizeof(int) * (2 * (size_t)nrows + CTL_N)));
     b->nrows_cap = nrows;
   }
+  if (nsb_total > b->trace_cap) {
+    cudaFree(b->trace); b->trace = nullptr; b->trace_cap = 0;
+    CK(cudaMalloc((void **)&b->trace, sizeof(tb_rdo_sb_trace_t) * nsb_total));
+    b->trace_cap = nsb_total;
+  }
   if (!b->ctl_host) CK(cudaMallocHost((void **)&b->ctl_host, sizeof(int) * CTL_N));
   int g = 0;
-  for (int s = 0; s < n_active; s++)
-    for (int r = 0; r < b->slots[s].nsby; r++) { b->rows_host[g].frame = s; b->rows_host[g].row = r; b->rows_host[g].nsbx = b->slots[s].nsbx; b->rows_host[g].pad = 0; g++; }
+  for (int s = 0; s < n_active; s++) {
+    const Slot &D = b->slots[s];
+    for (int r = 0; r < D.nsby; r++) { b->rows_host[g].frame = s; b->rows_host[g].row = r; b->rows_host[g].nsbx = D.nsbx; b->rows_host[g].path = D.nsbx + 2 * (D.nsby - 1 - r); g++; }
+  }
   b->nrows = nrows;
+  b->nsb = nsb_total;
   const size_t smem = smem_bytes<S>();
   static bool attr_set[3] = {false, false, false};
   static int per_sm[3] = {0, 0, 0};
@@ -849,7 +873,7 @@ template <class S> int batch_launch(tb_rdo_batch *b, int n_active, cudaStream_t 
   CK(cudaMemcpyAsync(b->sched_dev + 2 * (size_t)nrows, b->ctl_host, sizeof(int) * CTL_N, cudaMemcpyDefault, st));
   CK(cudaMemsetAsync(b->prof, 0, sizeof(unsigned long long) * ST_END, st));
   rdo_batch_kernel<S><<<grid, 32 * RDO_WARPS, smem, st>>>((const FrameCtx<S> *)b->ctx_dev, b->rows_dev, nrows, (Work<S> *)b->works, b->sched_dev, b->sched_dev + nrows,
-                                                         b->sched_dev + 2 * (size_t)nrows, b->prof);
+                                                         b->sched_dev + 2 * (size_t)nrows, b->prof, b->trace);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(b->ctl_host, b->sched_dev + 2 * (size_t)nrows, sizeof(int) * CTL_N, cudaMemcpyDefault, st));
   return TB_OK;
@@ -883,7 +907,7 @@ void tb_rdo_batch_destroy(tb_rdo_batch_t *b) {
   for (int s = 0; s < b->nslots; s++) b->slots[s].release();
   delete[] b->slots;
   cudaFreeHost(b->ctx_host); cudaFree(b->ctx_dev); cudaFreeHost(b->rows_host); cudaFree(b->rows_dev); cudaFree(b->sched_dev); cudaFreeHost(b->ctl_host);
-  cudaFree(b->works); cudaFree(b->prof);
+  cudaFree(b->works); cudaFree(b->prof); cudaFree(b->trace);
   delete b;
 }
 
@@ -986,6 +1010,14 @@ int tb_rdo_batch_stats(const tb_rdo_batch_t *b, uint64_t *out, int n) {
   if (!b || !out) return 0;
   const int m = n < TB_RDO_NSTATS ? n : TB_RDO_NSTATS;
   for (int k = 0; k < m; k++) out[k] = b->stats[k];
+  return m;
+}
+int tb_rdo_batch_trace(const tb_rdo_batch_t *b, tb_rdo_sb_trace_t *out, int n) {
+  if (!b) return 0;
+  if (!out) return b->nsb;
+  const int m = n < b->nsb ? n : b->nsb;
+  if (m <= 0) return 0;
+  CK(cudaMemcpy(out, b->trace, sizeof(tb_rdo_sb_trace_t) * m, cudaMemcpyDeviceToHost));
   return m;
 }
 

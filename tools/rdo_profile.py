@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """One launch of rdo_batch_kernel over the inter frames of a captured clip, for ncu / compute-sanitizer:
   ncu --set full --import-source on --clock-control none -k regex:rdo_batch -c 1 -o rdo python tools/rdo_profile.py --size 640x384
-Prints the kernel's own counters (cycles per primitive class, work executed)."""
+Prints the kernel's own counters (cycles per primitive class, work executed).  --copies 5 --size 1920x1080 is the launch bench.py times;
+--trace FILE writes the per-super-block timeline of the last launch (tb_rdo_batch_trace) as .npz for tools/rdo_sched.py."""
 import argparse
 import ctypes as C
 import json
@@ -24,6 +25,7 @@ def main():
     ap.add_argument("--copies", type=int, default=1)
     ap.add_argument("--launches", type=int, default=1)
     ap.add_argument("--cache", default="/tmp/thor_b200_bench")
+    ap.add_argument("--trace", default=None, metavar="FILE", help="write the per-super-block timeline of the last launch (.npz)")
     args = ap.parse_args()
     cfg = bench.Cfg(args.config, tuple(int(v) for v in args.size.split("x")), args.frames or None)
     os.makedirs(args.cache, exist_ok=True)
@@ -40,6 +42,7 @@ def main():
     L.tb_rdo_batch_sync.argtypes = [C.c_void_p]
     L.tb_rdo_batch_grid.argtypes = [C.c_void_p]
     L.tb_rdo_batch_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+    L.tb_rdo_batch_trace.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
     L.tb_rdo_last_error.restype = C.c_char_p
     jobs = [j for j in RJ.load_jobs(jobdir) if j.hdr.frame_type != 0]
     keep = []
@@ -47,7 +50,8 @@ def main():
     def alloc(n):
         a = np.zeros(max(n, 16), np.uint8); keep.append(a)
         return a.ctypes.data
-    hosts = [RJ.HostFrame(j, alloc) for _ in range(args.copies) for j in jobs]
+    base = [RJ.HostFrame(j, alloc) for j in jobs]  # copies upload from the same input planes
+    hosts = base + [RJ.HostFrame(j, alloc, share_inputs=hf) for _ in range(args.copies - 1) for j, hf in zip(jobs, base)]
     b = L.tb_rdo_batch_create(len(hosts), cfg.ESZ)
     for s, hf in enumerate(hosts):
         assert L.tb_rdo_batch_upload(b, s, C.byref(hf.desc)) == 0, L.tb_rdo_last_error()
@@ -68,6 +72,13 @@ def main():
            "cycles_per_prediction": round(d["cyc_interp"] / max(1, d["predictions"])), "cycles_per_intra": round(d["cyc_intra"] / max(1, d["intra_predictions"])),
            "warp_cycles_per_super_block": round(d["cyc_total"] * (1 - d["cyc_idle"] / max(1, d["cyc_total"])) / max(1, d["super_blocks"])),
            "share": {k[4:]: round(d[k] / max(1, d["cyc_total"]), 4) for k in bench.STAT_NAMES[:10] + bench.STAT_NAMES[23:40]}, "phase": {k[3:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[40:49])), 4) for k in bench.STAT_NAMES[40:49]}, "me_stage": {k[9:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[49:])), 4) for k in bench.STAT_NAMES[49:]}, "work": {k: d[k] for k in bench.STAT_NAMES[11:23]}}
+    if args.trace:
+        n = L.tb_rdo_batch_trace(b, None, 0)
+        tr = np.zeros(n, [(k, np.int32) for k in ("frame", "row", "col", "cta")] + [("t_start", np.uint64), ("t_end", np.uint64)])
+        assert L.tb_rdo_batch_trace(b, tr.ctypes.data, n) == n, L.tb_rdo_last_error()
+        sb = [1 << hf.desc.log2_sb_size for hf in hosts]
+        np.savez(args.trace, **{k: tr[k] for k in tr.dtype.names}, nsbx=np.array([-(-hf.desc.width // s) for hf, s in zip(hosts, sb)]),
+                 nsby=np.array([-(-hf.desc.height // s) for hf, s in zip(hosts, sb)]), ctas=out["ctas"])
     print(json.dumps(out))
 
 
