@@ -93,6 +93,51 @@ def rand_plane(rng, h, w, bitdepth, hbd, smooth=False):
     return a
 
 
+def rdo_hostcheck():
+    """oracle/librdo_hostcheck.so: tb_rdo.h over the plain-C oracle on the CPU (built by `make -C oracle port`, no reference sources needed).  It
+    exports tb_rdo_encode_frame like libthor_b200.so, so it is loaded through its own handle and never RTLD_GLOBAL."""
+    if "h" not in _cache:
+        so = os.path.join(ORACLE_DIR, "librdo_hostcheck.so")
+        if not os.path.exists(so):
+            subprocess.check_call(["make", "-s", "-C", ORACLE_DIR, "port"])
+        lib = C.CDLL(so, mode=C.RTLD_LOCAL)
+        lib.tb_rdo_encode_frame.argtypes = [C.c_void_p]
+        _cache["h"] = lib
+    return _cache["h"]
+
+
+def host_decisions(jobs, alloc, warps=1):
+    """every job decided by rdo_hostcheck() into fresh RJ.HostFrame buffers, frame by frame, with `warps` simulated warps (TBR_HOST_WARPS)"""
+    from thor_b200 import rdo_jobs as RJ
+    lib = rdo_hostcheck()
+    old = os.environ.get("TBR_HOST_WARPS")
+    os.environ["TBR_HOST_WARPS"] = str(warps)
+    try:
+        hosts = [RJ.HostFrame(j, alloc) for j in jobs]
+        for hf in hosts:
+            assert lib.tb_rdo_encode_frame(C.byref(hf.desc)) == 0
+    finally:
+        if old is None:
+            del os.environ["TBR_HOST_WARPS"]
+        else:
+            os.environ["TBR_HOST_WARPS"] = old
+    return hosts
+
+
+def host_decisions_of_dir(directory):
+    """host_decisions() of the jobs in `directory`, as plain arrays for another process: [(check(), leaves, leaf_count, coeffs)] per frame"""
+    import sys
+    if ROOT not in sys.path:  # a spawned worker process
+        sys.path.insert(0, ROOT)
+    from thor_b200 import rdo_jobs as RJ
+    keep = []
+
+    def alloc(nbytes):
+        a = np.zeros(max(nbytes, 16), np.uint8); keep.append(a)
+        return a.ctypes.data
+    return [(hf.check(), hf.leaves.copy(), hf.leaf_count.copy(), hf.coeffs.copy()) for hf in host_decisions(RJ.load_jobs(directory), alloc)]
+
+
 def ref_frame(hbd):
     """oracle/_ref/libthorref_frame_{lbd,hbd}.so: cdef_search + dist_8x8 trampolines (enc/encode_frame.c included in place)"""
     k = "rf%d" % hbd

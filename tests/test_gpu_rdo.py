@@ -8,20 +8,27 @@ import subprocess
 import pytest
 
 from test_dropin_link import HDB, LDB, REF, synth_yuv
+from test_rdo_matrix import hard_yuv
 
 needs = pytest.mark.skipif(not (os.path.exists(os.path.join(REF, "Thorenc_b200_rdo")) and os.path.exists(os.path.join(REF, "Thorenc"))),
                            reason="oracle/_ref (reference objects + drop-in links) not built")
 
 
-def enc(exe, flags, w, h, n, tag, tmp, extra, env=None):
+def enc(exe, flags, w, h, n, tag, tmp, extra, env=None, qp=32):
+    """encode tmp/in.yuv (written by the caller) with oracle/_ref/<exe>"""
     bit, rec = os.path.join(tmp, tag + ".bit"), os.path.join(tmp, tag + "_rec.yuv")
-    cmd = [os.path.join(REF, exe)] + flags + ["-if", os.path.join(tmp, "in.yuv"), "-of", bit, "-rf", rec, "-width", str(w), "-height", str(h), "-n", str(n), "-qp", "32",
+    cmd = [os.path.join(REF, exe)] + flags + ["-if", os.path.join(tmp, "in.yuv"), "-of", bit, "-rf", rec, "-width", str(w), "-height", str(h), "-n", str(n), "-qp", str(qp),
                                               "-f", "30"] + list(extra)
     e = dict(os.environ)
     e.update(env or {})
     r = subprocess.run(cmd, capture_output=True, text=True, timeout=1500, env=e)
     assert r.returncode == 0, (r.stdout[-1500:], r.stderr[-2000:])
     return open(bit, "rb").read(), open(rec, "rb").read(), r.stderr, bit
+
+
+# qp and clip of the cases that do not encode synth_yuv at qp 32: low qp on 10-bit hard content (large coefficients, saturation), nearly everything
+# skipped (qp 51), cfl_inter, encoder speed 1 on a frame narrower than two super blocks
+CLIPS = {"hdb_10bit_q4_hard": (4, hard_yuv), "hdb_8bit_q51": (51, synth_yuv), "hdb_8bit_cfl_inter_hard": (22, hard_yuv), "hdb_8bit_speed1_rect_hard": (8, hard_yuv)}
 
 
 @pytest.mark.gpu
@@ -32,12 +39,18 @@ def enc(exe, flags, w, h, n, tag, tmp, extra, env=None):
     ("hdb_10bit_B", HDB + ["-cdef", "0"], 128, 136, 9, ("-bitdepth", "10", "-input_bitdepth", "10"), True),
     ("hdb_8bit_rect", HDB + ["-cdef", "0"], 200, 136, 3, (), True),   # widths that are not a multiple of the super block: rectangular skips
     ("hdb_8bit_cdef", HDB, 256, 192, 9, (), False),                   # CDEF on (tiny-frame streams are undecodable in the reference, SURVEY §8c.3: encoder outputs only)
+    # cases of tests/test_rdo_matrix.py, with their qp and clip in CLIPS
+    ("hdb_10bit_q4_hard", HDB + ["-cdef", "0"], 128, 136, 5, ("-bitdepth", "10", "-input_bitdepth", "10"), True),
+    ("hdb_8bit_q51", HDB + ["-cdef", "0"], 128, 136, 9, (), True),
+    ("hdb_8bit_cfl_inter_hard", HDB + ["-cdef", "0", "-enable_cfl_inter", "1"], 128, 136, 5, (), True),
+    ("hdb_8bit_speed1_rect_hard", HDB + ["-cdef", "0", "-encoder_speed", "1"], 200, 72, 5, (), True),
 ])
 def test_device_rd_loop_encode_is_bit_exact(tmp_path, name, flags, w, h, n, extra, decode):
     tmp = str(tmp_path)
-    synth_yuv(os.path.join(tmp, "in.yuv"), w, h, n, 10 if "10bit" in name else 8)
-    bit_ref, rec_ref, _, _ = enc("Thorenc", flags, w, h, n, "ref", tmp, extra)
-    bit, rec, err, bitfile = enc("Thorenc_b200_rdo", flags, w, h, n, "gpu", tmp, extra, {"TB_RDO_STATS": "1"})
+    qp, make_clip = CLIPS.get(name, (32, synth_yuv))
+    make_clip(os.path.join(tmp, "in.yuv"), w, h, n, 10 if "10bit" in name else 8)
+    bit_ref, rec_ref, _, _ = enc("Thorenc", flags, w, h, n, "ref", tmp, extra, qp=qp)
+    bit, rec, err, bitfile = enc("Thorenc_b200_rdo", flags, w, h, n, "gpu", tmp, extra, {"TB_RDO_STATS": "1"}, qp=qp)
     assert "frames decided by tb_rdo_encode_frame: %d," % n in err, err[-800:]   # every frame went through the device RD loop (no host-loop frames)
     assert bit == bit_ref, "bitstream differs"
     assert rec == rec_ref, "reconstruction differs"

@@ -29,9 +29,10 @@ CASES = [
 ]
 
 
-def enc(exe, flags, w, h, n, tag, tmp, extra, env=None):
+def enc(exe, flags, w, h, n, tag, tmp, extra, env=None, qp=32):
+    """encode tmp/in.yuv (written by the caller) with oracle/_ref/<exe>"""
     bit, rec = os.path.join(tmp, tag + ".bit"), os.path.join(tmp, tag + "_rec.yuv")
-    cmd = [os.path.join(REF, exe)] + flags + ["-if", os.path.join(tmp, "in.yuv"), "-of", bit, "-rf", rec, "-width", str(w), "-height", str(h), "-n", str(n), "-qp", "32",
+    cmd = [os.path.join(REF, exe)] + flags + ["-if", os.path.join(tmp, "in.yuv"), "-of", bit, "-rf", rec, "-width", str(w), "-height", str(h), "-n", str(n), "-qp", str(qp),
                                               "-f", "30"] + list(extra)
     e = dict(os.environ)
     e.update(env or {})

@@ -16,13 +16,14 @@ needs = pytest.mark.skipif(not (os.path.exists(os.path.join(REF, "Thorenc_captur
                            reason="oracle/_ref (reference objects + capture link) not built")
 
 
-def capture(tmp, flags, w, h, n, bitdepth=8):
+def capture(tmp, flags, w, h, n, bitdepth=8, qp=32, make_clip=synth_yuv):
+    """encode make_clip(path, w, h, n, bitdepth) with the reference encoder and with the capture link; returns the directory of the captured jobs"""
     clip = os.path.join(tmp, "in.yuv")
-    synth_yuv(clip, w, h, n, bitdepth)
+    make_clip(clip, w, h, n, bitdepth)
     jobs = os.path.join(tmp, "jobs")
     os.makedirs(jobs, exist_ok=True)
     extra = ["-bitdepth", str(bitdepth), "-input_bitdepth", str(bitdepth)] if bitdepth != 8 else []
-    common = ["-if", clip, "-width", str(w), "-height", str(h), "-n", str(n), "-qp", "32", "-f", "30"] + extra
+    common = ["-if", clip, "-width", str(w), "-height", str(h), "-n", str(n), "-qp", str(qp), "-f", "30"] + extra
     r0 = subprocess.run([os.path.join(REF, "Thorenc")] + flags + common + ["-of", os.path.join(tmp, "a.bit"), "-rf", os.path.join(tmp, "a.yuv")], capture_output=True, text=True)
     r1 = subprocess.run([os.path.join(REF, "Thorenc_capture")] + flags + common + ["-of", os.path.join(tmp, "b.bit"), "-rf", os.path.join(tmp, "b.yuv")], capture_output=True,
                         text=True, env=dict(os.environ, TB_RDO_DUMP=jobs, TB_RDO_STATS="1"))
@@ -78,39 +79,33 @@ def test_batched_rd_loop_equals_reference_decisions(tmp_path, name, flags, w, h,
         assert r == {"rec": True, "blk": True, "sb_cost": True}, (name, "frame", hf.job.frame_num, "copy", k // len(jobs), r)
 
 
-# ---- committed golden jobs (tests/golden/rdo_jobs_hdb_128x136.xz, generated from the reference by tests/golden/make_golden_rdo.py)
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "rdo_jobs_hdb_128x136.xz")
+# ---- committed golden jobs (tests/golden/rdo_jobs_*.xz, generated from the reference by tests/golden/make_golden_rdo.py):
+#   hdb_128x136        9 frames of 128x136 HDB at qp 32 on smooth content (I, P, seven hierarchical B frames)
+#   hdb_hard_q4_10bit  5 frames of 128x136 10-bit HDB at qp 4 on tests/test_rdo_matrix.py:hard_yuv (large coefficients, saturated samples)
+GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+GOLDEN_FRAMES = {"hdb_128x136": 9, "hdb_hard_q4_10bit": 5}
 
 
-def golden_jobs(tmp):
+def golden_module():
     import importlib.util
-    spec = importlib.util.spec_from_file_location("make_golden_rdo", os.path.join(os.path.dirname(GOLDEN), "make_golden_rdo.py"))
+    spec = importlib.util.spec_from_file_location("make_golden_rdo", os.path.join(GOLDEN_DIR, "make_golden_rdo.py"))
     m = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(m)
-    n = m.unpack(open(GOLDEN, "rb").read(), tmp)
+    return m
+
+
+def golden_jobs(tmp, case="hdb_128x136"):
+    m = golden_module()
+    n = m.unpack(open(m.path(case), "rb").read(), tmp)
     return m, n
 
 
-@needs
-def test_golden_rdo_jobs_are_what_the_reference_writes_today(tmp_path):
-    """the fixture is pinned: a fresh capture with the compiled reference reproduces it byte for byte"""
-    m, n = golden_jobs(str(tmp_path))
-    fresh_dir = tmp_path / "fresh"
-    fresh_dir.mkdir()
-    fresh = m.capture(str(fresh_dir))
-    assert n == len(fresh) == 9
-    for k in range(n):
-        assert open(os.path.join(str(tmp_path), "frame_%03d.job" % k), "rb").read() == fresh[k], "job %d differs from a fresh capture" % k
-
-
-@pytest.mark.gpu
-def test_batched_rd_loop_on_the_golden_jobs(tmp_path):
-    """the device RD loop against the committed decisions of the reference (no oracle/_ref needed on the GPU box): all nine frames in one launch"""
+def decide_and_check(jobs):
+    """all jobs in one tb_rdo_encode_frames() launch; every frame must return the reference's reconstruction, block state and cost per super block,
+    and code exactly as oracle/librdo_hostcheck.so's decisions on the same job (leaf lists and coefficients, RJ.leaf_differences)"""
     import thor_b200 as tb
     from thor_b200 import rdo_jobs as RJ
-    golden_jobs(str(tmp_path))
-    jobs = RJ.load_jobs(str(tmp_path))
-    assert len(jobs) == 9 and [j.hdr.frame_type for j in jobs].count(2) == 7
+    from _libs import host_decisions
     L = tb.lib
     L.tb_rdo_encode_frames.argtypes = [C.c_void_p, C.c_int]
     L.tb_rdo_last_error.restype = C.c_char_p
@@ -123,4 +118,70 @@ def test_batched_rd_loop_on_the_golden_jobs(tmp_path):
     descs = (RJ.RdoFrame * len(hosts))(*[hf.desc for hf in hosts])
     assert L.tb_rdo_encode_frames(descs, len(hosts)) == 0, L.tb_rdo_last_error()
     for hf in hosts:
-        assert hf.check() == {"rec": True, "blk": True, "sb_cost": True}, ("frame", hf.job.frame_num)
+        assert hf.check() == {"rec": True, "blk": True, "sb_cost": True}, ("frame", hf.job.frame_num, hf.check())
+    for hf, want in zip(hosts, host_decisions(jobs, alloc)):
+        assert want.check() == {"rec": True, "blk": True, "sb_cost": True}, ("frame", hf.job.frame_num, "host decisions differ from the reference's")
+        d = hf.leaf_differences(want)
+        assert not d, ("frame", hf.job.frame_num, d)
+
+
+def rederive(tmp_path, case):
+    m, n = golden_jobs(str(tmp_path), case)
+    fresh_dir = tmp_path / "fresh"
+    fresh_dir.mkdir()
+    fresh = m.capture(str(fresh_dir), case)
+    assert n == len(fresh) == GOLDEN_FRAMES[case]
+    for k in range(n):
+        assert open(os.path.join(str(tmp_path), "frame_%03d.job" % k), "rb").read() == fresh[k], "job %d differs from a fresh capture" % k
+
+
+@needs
+def test_golden_rdo_jobs_are_what_the_reference_writes_today(tmp_path):
+    """the fixture is pinned: a fresh capture with the compiled reference reproduces it byte for byte"""
+    rederive(tmp_path, "hdb_128x136")
+
+
+@needs
+def test_hard_low_qp_golden_rdo_jobs_are_what_the_reference_writes_today(tmp_path):
+    rederive(tmp_path, "hdb_hard_q4_10bit")
+
+
+@pytest.mark.parametrize("case", sorted(GOLDEN_FRAMES))
+def test_host_decisions_of_the_golden_jobs_code_alike_with_any_warp_count(tmp_path, case):
+    """oracle/librdo_hostcheck.so (tb_rdo.h over the oracle; no reference needed) returns the reference's decisions on the committed jobs, and
+    its leaf lists and coefficients code identically with one and with eight simulated warps: what RJ.leaf_differences compares does not depend on
+    which warp evaluated which candidate, so it can compare the device's eight-warp decisions with the host's"""
+    from thor_b200 import rdo_jobs as RJ
+    from _libs import host_decisions
+    golden_jobs(str(tmp_path), case)
+    jobs = RJ.load_jobs(str(tmp_path))
+    keep = []
+
+    def alloc(nbytes):
+        a = np.zeros(max(nbytes, 16), np.uint8); keep.append(a)
+        return a.ctypes.data
+    one, eight = host_decisions(jobs, alloc, warps=1), host_decisions(jobs, alloc, warps=8)
+    for a, b in zip(one, eight):
+        assert a.check() == b.check() == {"rec": True, "blk": True, "sb_cost": True}, ("frame", a.job.frame_num)
+        assert a.leaf_count.sum() > 0
+        assert not b.leaf_differences(a), ("frame", a.job.frame_num, b.leaf_differences(a))
+
+
+@pytest.mark.gpu
+def test_batched_rd_loop_on_the_golden_jobs(tmp_path):
+    """the device RD loop against the committed decisions of the reference (no oracle/_ref needed on the GPU box): all nine frames in one launch"""
+    from thor_b200 import rdo_jobs as RJ
+    golden_jobs(str(tmp_path))
+    jobs = RJ.load_jobs(str(tmp_path))
+    assert len(jobs) == 9 and [j.hdr.frame_type for j in jobs].count(2) == 7
+    decide_and_check(jobs)
+
+
+@pytest.mark.gpu
+def test_batched_rd_loop_on_the_hard_low_qp_golden_jobs(tmp_path):
+    """the same on the 10-bit qp 4 hard-content fixture: large coefficients, saturated samples, a scene cut and local motion"""
+    from thor_b200 import rdo_jobs as RJ
+    golden_jobs(str(tmp_path), "hdb_hard_q4_10bit")
+    jobs = RJ.load_jobs(str(tmp_path))
+    assert len(jobs) == 5 and all(j.hdr.bitdepth == 10 and j.hdr.qp <= 8 for j in jobs)
+    decide_and_check(jobs)

@@ -1,0 +1,200 @@
+"""The RD loop across the quantiser range, hard content and encoder options.
+
+One table of cases (CASES) drives every test here:
+  CPU  oracle/_ref/Thorenc_rdocheck with TB_RDO_VERIFY=1: every super block of every case, decided by thor_b200/csrc/tb_rdo.h over the plain-C
+       oracle and by the reference's process_block() on the same encoder state, must be identical; two cases also run with eight simulated warps.
+  GPU  every case captured with the reference (oracle/_ref/Thorenc_capture); all 8-bit frames of all cases decided in ONE tb_rdo_encode_frames()
+       launch, all 10-bit frames in a second one.  Frames of one launch differ in size, qp, speed and options.  Every frame must return the
+       reference's reconstruction, block state and cost per super block, and the leaf lists and coefficients that oracle/librdo_hostcheck.so
+       (tb_rdo.h over the oracle, itself checked against the reference first) returns for the same job: everything the bit writer reads.
+The cases reach what qp 32 on smooth content does not: large coefficients and saturation in the transform chain (low qp), frames that are nearly
+all skipped (qp 51), samples at 0 and 2^bd-1 in prediction, bipred average and reconstruction, intra blocks in inter frames (a scene cut), local
+motion, cfl_inter, encoder speeds 1 and 3, block contexts off, no tb split, intra_rdo 0, no early skip and two references."""
+import ctypes as C
+import os
+import re
+from concurrent.futures import ThreadPoolExecutor
+
+import numpy as np
+import pytest
+
+from test_dropin_link import HDB, LDB, REF, synth_yuv
+
+
+def hard_yuv(path, w, h, n, bitdepth=8, seed=11):
+    """Seeded 4:2:0 content at the edges of the RD loop:
+      * luma: a uniform-noise texture that pans by one row and one column per frame (motion search finds it; every residual is large);
+      * the bottom-right quadrant: a second noise texture moving by (-3, +2) per frame, against the background;
+      * a 24x24 block at (16, 16) that alternates between 0 and 2^bd-1 every frame;
+      * frame n // 2 + 1 (when n > 2): fresh noise everywhere, a scene cut;
+      * U: uniform noise; V: every sample either 0 or 2^bd-1."""
+    rng = np.random.default_rng(seed)
+    maxv = (1 << bitdepth) - 1
+    m = 4 * n + 8
+    bg = rng.integers(0, maxv + 1, (h + m, w + m))
+    fg = rng.integers(0, maxv + 1, (h + m, w + m))
+    cut = n // 2 + 1 if n > 2 else -1
+    qy, qx = h // 2, w // 2
+    with open(path, "wb") as f:
+        for k in range(n):
+            y = bg[k:k + h, k:k + w].copy()
+            y[qy:, qx:] = fg[3 * k:3 * k + h - qy, 2 * (n - k):2 * (n - k) + w - qx]
+            y[16:40, 16:40] = maxv if k % 2 else 0
+            if k == cut:
+                y = rng.integers(0, maxv + 1, (h, w))
+            u = rng.integers(0, maxv + 1, (h // 2, w // 2))
+            v = rng.integers(0, 2, (h // 2, w // 2)) * maxv
+            for p in (y, u, v):
+                f.write(p.astype(np.uint8 if bitdepth == 8 else "<u2").tobytes())
+
+
+CONTENT = {"synth": synth_yuv, "hard": hard_yuv}
+HDB0 = HDB + ["-cdef", "0"]   # tiny frames + CDEF corrupt the reference's header (SURVEY §8c.3)
+CASES = [
+    # name               flags                                                         w    h    frames qp bitdepth content
+    ("hdb_q4",           HDB0,                                                         128, 136, 9, 4,  8,  "synth"),
+    ("hdb_q51",          HDB0,                                                         128, 136, 9, 51, 8,  "synth"),
+    ("hdb_q12_hard",     HDB0,                                                         128, 136, 9, 12, 8,  "hard"),
+    ("hdb_q4_hard_10",   HDB0,                                                         128, 136, 5, 4,  10, "hard"),
+    ("hdb_q51_hard_10",  HDB0,                                                         128, 136, 5, 51, 10, "hard"),
+    ("hdb_q32_hard",     HDB0,                                                         128, 136, 9, 32, 8,  "hard"),
+    ("cfl_inter",        HDB0 + ["-enable_cfl_inter", "1"],                            128, 136, 9, 32, 8,  "synth"),
+    ("cfl_inter_hard",   HDB0 + ["-enable_cfl_inter", "1"],                            128, 136, 5, 22, 8,  "hard"),
+    ("speed1",           HDB0 + ["-encoder_speed", "1"],                               128, 136, 9, 32, 8,  "synth"),
+    ("speed1_hard_rect", HDB0 + ["-encoder_speed", "1"],                               200, 72,  5, 8,  8,  "hard"),
+    ("speed3",           HDB0 + ["-encoder_speed", "3"],                               128, 136, 9, 32, 8,  "synth"),
+    ("no_ctx_no_tbsplit", HDB0 + ["-use_block_contexts", "0", "-enable_tb_split", "0"], 128, 136, 9, 32, 8,  "synth"),
+    ("intra_rdo0",       HDB0 + ["-intra_rdo", "0"],                                   128, 136, 9, 32, 8,  "synth"),
+    ("no_bipred_hard",   HDB0 + ["-enable_bipred", "0"],                               128, 136, 9, 32, 8,  "hard"),
+    ("max_ref2",         HDB0 + ["-max_num_ref", "2"],                                 128, 136, 9, 32, 8,  "synth"),
+    ("no_early_skip",    HDB0 + ["-early_skip_thr", "0"],                              128, 136, 9, 32, 8,  "synth"),
+    ("ldb_q45_hard",     LDB,                                                          256, 136, 4, 45, 8,  "hard"),
+]
+BY_NAME = {c[0]: c for c in CASES}
+
+
+def write_clip(tmp, case):
+    name, flags, w, h, n, qp, bd, content = case
+    CONTENT[content](os.path.join(tmp, "in.yuv"), w, h, n, bd)
+    return ("-bitdepth", str(bd), "-input_bitdepth", str(bd)) if bd != 8 else ()
+
+
+def super_blocks(w, h, n):
+    return ((w + 127) // 128) * ((h + 127) // 128) * n
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------------------------
+# CPU: tb_rdo.h over the oracle against the reference's process_block, super block by super block
+# ---------------------------------------------------------------------------------------------------------------------------------------------------
+needs_check = pytest.mark.skipif(not (os.path.exists(os.path.join(REF, "Thorenc_rdocheck")) and os.path.exists(os.path.join(REF, "Thorenc"))),
+                                 reason="oracle/_ref/Thorenc_rdocheck not built (make -C oracle ref rdocheck)")
+
+
+def verify(tmp, case, env=()):
+    from test_rdo_host import enc
+    name, flags, w, h, n, qp, bd, content = case
+    extra = write_clip(tmp, case)
+    _, _, err = enc("Thorenc_rdocheck", flags, w, h, n, "chk", tmp, extra, dict({"TB_RDO_VERIFY": "1", "TB_RDO_VERBOSE": "1"}, **dict(env)), qp=qp)
+    m = re.search(r"verify: (\d+) super blocks compared with the reference's process_block, (\d+) differ", err)
+    assert m, err[-1500:]
+    assert (int(m.group(1)), int(m.group(2))) == (super_blocks(w, h, n), 0), err[-3000:]
+
+
+@needs_check
+@pytest.mark.parametrize("case", CASES, ids=[c[0] for c in CASES])
+def test_every_super_block_matches_reference_process_block(tmp_path, case):
+    verify(str(tmp_path), case)
+
+
+@needs_check
+@pytest.mark.parametrize("name", ["cfl_inter_hard", "hdb_q4_hard_10"])
+def test_overlapped_decision_with_the_device_warp_count(tmp_path, name):
+    """the device decides with eight warps per CTA; host threads stand in for them (TBR_HOST_WARPS), see tests/test_rdo_host.py"""
+    verify(str(tmp_path), BY_NAME[name], {"TBR_HOST_WARPS": "8"})
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------------------------
+# GPU: all cases in one launch per sample size
+# ---------------------------------------------------------------------------------------------------------------------------------------------------
+needs_capture = pytest.mark.skipif(not (os.path.exists(os.path.join(REF, "Thorenc_capture")) and os.path.exists(os.path.join(REF, "Thorenc"))),
+                                   reason="oracle/_ref (reference objects + capture link) not built")
+
+
+def alloc_into(keep):
+    def alloc(nbytes):
+        a = np.zeros(max(nbytes, 16), np.uint8); keep.append(a)
+        return a.ctypes.data
+    return alloc
+
+
+@pytest.fixture(scope="module")
+def matrix_jobs(tmp_path_factory):
+    """every case captured with the reference encoder: {name: (job directory, jobs)}"""
+    from test_rdo_jobs import capture
+    from thor_b200 import rdo_jobs as RJ
+
+    def one(case):
+        name, flags, w, h, n, qp, bd, content = case
+        d = str(tmp_path_factory.mktemp(name))
+        jobdir = capture(d, flags, w, h, n, bd, qp, CONTENT[content])
+        return name, (jobdir, RJ.load_jobs(jobdir))
+    with ThreadPoolExecutor(min(8, os.cpu_count() or 1)) as ex:
+        return dict(ex.map(one, CASES))
+
+
+@pytest.fixture(scope="module")
+def launches(matrix_jobs):
+    """launch(bitdepth) -> (return code, [(case name, device HostFrame)]): the frames of every case with that bit depth in one tb_rdo_encode_frames()
+    call, each launch made once per module"""
+    import thor_b200 as tb
+    from thor_b200 import rdo_jobs as RJ
+    L = tb.lib
+    L.tb_rdo_encode_frames.argtypes = [C.c_void_p, C.c_int]
+    L.tb_rdo_last_error.restype = C.c_char_p
+    done, keep = {}, []
+
+    def launch(bd):
+        if bd not in done:
+            hosts = [(c[0], RJ.HostFrame(j, alloc_into(keep))) for c in CASES if c[6] == bd for j in matrix_jobs[c[0]][1]]
+            descs = (RJ.RdoFrame * len(hosts))(*[hf.desc for _, hf in hosts])
+            rc = L.tb_rdo_encode_frames(descs, len(hosts))
+            done[bd] = (rc, hosts, L.tb_rdo_last_error() if rc else b"")
+        return done[bd]
+    return launch
+
+
+@pytest.mark.gpu
+@needs_capture
+@pytest.mark.parametrize("bd", [8, 10])
+def test_matrix_in_one_launch_equals_reference_decisions(launches, bd):
+    rc, hosts, err = launches(bd)
+    assert rc == 0, err
+    assert len({(hf.job.hdr.width, hf.job.hdr.height, hf.job.hdr.qp, hf.job.hdr.encoder_speed) for _, hf in hosts}) > 1  # parameters differ within the launch
+    bad = [(name, hf.job.frame_num, r) for name, hf in hosts for r in [hf.check()] if not all(r.values())]
+    assert not bad, "%d of %d frames differ from the reference: %s" % (len(bad), len(hosts), bad[:8])
+
+
+@pytest.mark.gpu
+@needs_capture
+@pytest.mark.parametrize("bd", [8, 10])
+def test_matrix_leaf_lists_and_coefficients_equal_host_decisions(launches, matrix_jobs, bd):
+    import multiprocessing
+    from concurrent.futures import ProcessPoolExecutor
+    from _libs import host_decisions_of_dir
+    from thor_b200 import rdo_jobs as RJ
+    rc, hosts, err = launches(bd)
+    assert rc == 0, err
+    names = [c[0] for c in CASES if c[6] == bd]
+    # the host decisions of each case in a process of its own (the CPU side takes about a second per frame)
+    with ProcessPoolExecutor(min(8, os.cpu_count() or 1), mp_context=multiprocessing.get_context("spawn")) as ex:
+        want = dict(zip(names, ex.map(host_decisions_of_dir, [matrix_jobs[n][0] for n in names])))
+    bad = []
+    for name in names:
+        got = [hf for n, hf in hosts if n == name]
+        assert len(got) == len(want[name])
+        for g, (check, leaves, count, coeffs) in zip(got, want[name]):
+            assert check == {"rec": True, "blk": True, "sb_cost": True}, (name, "frame", g.job.frame_num, "host decisions differ from the reference's")
+            d = RJ.leaf_differences(g.leaves, g.leaf_count, g.coeffs, leaves, count, coeffs)
+            if d:
+                bad.append((name, g.job.frame_num, d))
+    assert not bad, "%d frames code differently from the host decisions; first: %s" % (len(bad), bad[:3])

@@ -51,6 +51,69 @@ def leaf_coeffs(leaf, coeffs):
     return coeffs[ofs:ofs + coeff_count(size, split) + 2 * coeff_count(sc, int(split and sc > 4))]
 
 
+# Which leaf fields the reference's bit writer reads, per block mode (SKIP 0, INTRA 1, INTER 2, BIPRED 3, MERGE 4), with the lines of enc/write_bits.c that
+# read them (write_super_mode :257-358, write_block :360-600; tb_rdo_shim.c emit_node hands every field to them).  Outside these modes a field holds
+# whichever candidate state the deciding warp held last, so two correct decisions may differ there.  `dir` is not read by the bit writer at all.
+ALL_MODES = (0, 1, 2, 3, 4)
+LEAF_FIELD_MODES = {
+    "xpos": ALL_MODES, "ypos": ALL_MODES, "size": ALL_MODES,   # emit_node matches the leaf to its quad-tree node by position and size
+    "mode": ALL_MODES,                                          # :291-349 mode code
+    "cost": ALL_MODES,                                          # not written: the RD cost the super block's decisions add up to
+    "coeff_ofs": ALL_MODES,                                     # where emit_node unpacks coeff_y/u/v from (-1: none)
+    "ctx_index": ALL_MODES,                                     # :284, :315, :344 mode code order
+    "intra_mode": (1,),                                         # :395-401
+    "pb_part": (2, 3),                                          # :405-406, :410-429 (INTER); :441-465 which mv_arr1 entries (BIPRED)
+    "mv_arr0": (2, 3),                                          # :410-429 (INTER); :441-445 (BIPRED)
+    "mv_arr1": (3,),                                            # :446-465
+    "mvp": (2, 3),                                              # :409, :440
+    "ref_idx0": (2, 3),                                         # :300-304, :324-333 (INTER); :467-474 (BIPRED in P frames)
+    "ref_idx1": (3,),                                           # :467-474
+    "skip_idx": (0, 4),                                         # :477-498
+    "num_skip_vec": (0,),                                       # :479-486
+    "num_merge_vec": (4,),                                      # :490-497
+    "ctx_cbp": (1, 2, 3, 4),                                    # :522, :551
+    "tb_split": (1, 2, 3, 4),                                   # :509, :530, :542-594
+    "cbp_y": (1, 2, 3, 4), "cbp_u": (1, 2, 3, 4), "cbp_v": (1, 2, 3, 4),   # :513-540, :545-591
+}
+# the motion vectors write_mv codes per pb_part (PART_NONE, PART_HOR, PART_VER, PART_QUAD): :410-428 and :446-464; BIPRED codes mv_arr0[0] only (:441-442)
+MV_ENTRIES = {0: (0,), 1: (0, 2), 2: (0, 1), 3: (0, 1, 2, 3)}
+
+
+def leaf_differences(got_leaves, got_count, got_coeffs, want_leaves, want_count, want_coeffs, limit=8):
+    """what the bit writer would code differently from `got` than from `want` (one frame): leaf counts per super block, the fields of
+    LEAF_FIELD_MODES where the block's mode reads them, and the quantised coefficients each leaf references.  Returns up to `limit` descriptions
+    (super block, leaf index, position, mode, field, got, want), first difference first; empty when the frames code identically."""
+    out = []
+    for s in range(len(want_count)):
+        if got_count[s] != want_count[s]:
+            out.append("sb %d: leaf_count %d, want %d" % (s, got_count[s], want_count[s]))
+            if len(out) >= limit:
+                return out
+            continue
+        for i in range(int(want_count[s])):
+            g, w = got_leaves[s, i], want_leaves[s, i]
+            mode = int(w["mode"])
+            where = "sb %d leaf %d (x %d y %d size %d mode %d)" % (s, i, w["xpos"], w["ypos"], w["size"], mode)
+            for name, modes in LEAF_FIELD_MODES.items():
+                if mode not in modes:
+                    continue
+                gv, wv = g[name], w[name]
+                if name in ("mv_arr0", "mv_arr1"):
+                    pb = int(w["pb_part"])
+                    idx = (0,) if (name == "mv_arr0" and mode == 3) else MV_ENTRIES.get(pb, MV_ENTRIES[3])
+                    gv, wv = gv[list(idx)], wv[list(idx)]
+                if not np.array_equal(gv, wv):
+                    out.append("%s: %s %s, want %s" % (where, name, np.asarray(gv).tolist(), np.asarray(wv).tolist()))
+            if int(w["coeff_ofs"]) >= 0 and int(g["coeff_ofs"]) == int(w["coeff_ofs"]):
+                gc, wc = leaf_coeffs(w, got_coeffs[s]), leaf_coeffs(w, want_coeffs[s])
+                if not np.array_equal(gc, wc):
+                    k = int(np.flatnonzero(gc != wc)[0])
+                    out.append("%s: coefficient %d of %d is %d, want %d" % (where, k, wc.size, gc[k], wc[k]))
+            if len(out) >= limit:
+                return out[:limit]
+    return out
+
+
 class Job:
     """one frame_NNN.job: .hdr (RdoFrame with NULL pointers), .frame_num, .nsb, .orig[3], .refs[r][3] (whole padded planes), and the reference's
     results .rec[3], .blk, .sb_cost"""
@@ -161,3 +224,7 @@ class HostFrame:
         cost = np.array([int(self.leaves["cost"][s, :self.leaf_count[s]].astype(np.int64).sum()) for s in range(j.nsb)], dtype=np.int64)
         cost_ok = np.array_equal(cost, j.sb_cost.astype(np.int64))
         return {"rec": bool(rec_ok), "blk": bool(blk_ok), "sb_cost": bool(cost_ok)}
+
+    def leaf_differences(self, want, limit=8):
+        """leaf_differences() of this frame's leaf lists and coefficients against those of `want`, a HostFrame of the same job"""
+        return leaf_differences(self.leaves, self.leaf_count, self.coeffs, want.leaves, want.leaf_count, want.coeffs, limit)
