@@ -18,12 +18,14 @@ typedef struct {
   tb_frame_t *rec, *scratch, *ref_out;
   tb_blkinfo_t *bi_host, *bi_dev;
   int8_t *fb_pri_dev[2], *fb_sec_dev[2];
+  uint8_t *clpf_fb_on_dev;
   int32_t *dirvar_dev;
-  int nblk, nfb;
+  int width, height, nblk, nfb;
 } tb_filter_ctx;
 
 /* once per sequence */
 int tb_filter_ctx_create(tb_filter_ctx *c, int width, int height) {
+  c->width = width; c->height = height;
   c->nblk = (width / MIN_PB_SIZE) * (height / MIN_PB_SIZE);
   c->nfb = ((width + 63) / 64) * ((height + 63) / 64);
   c->rec = tb_frame_create(width, height, PADDING_Y, (int)sizeof(SAMPLE));
@@ -35,15 +37,19 @@ int tb_filter_ctx_create(tb_filter_ctx *c, int width, int height) {
     c->fb_pri_dev[k] = (int8_t *)tb_malloc((size_t)c->nfb);
     c->fb_sec_dev[k] = (int8_t *)tb_malloc((size_t)c->nfb);
   }
+  c->clpf_fb_on_dev = (uint8_t *)tb_malloc((size_t)((width + 15) / 16) * ((height + 15) / 16)); /* the smallest signalled CLPF block is 16x16 */
   c->dirvar_dev = (int32_t *)tb_malloc((size_t)c->nfb * 2 * 64 * sizeof(int32_t));
-  return c->rec && c->scratch && c->ref_out && c->bi_host && c->bi_dev && c->dirvar_dev ? TB_OK : TB_ERR_CUDA;
+  return c->rec && c->scratch && c->ref_out && c->bi_host && c->bi_dev && c->clpf_fb_on_dev && c->dirvar_dev ? TB_OK : TB_ERR_CUDA;
 }
 
 /* per frame: replaces deblock_frame_y/_uv, cdef_frame x3, clpf_frame x3 and create_reference_frame (enc/encode_frame.c:748-835).
  * fb_pri / fb_sec: per 64x64 filter block, [0] luma, [1] chroma — cdef_strength.level / .sec_strength as chosen by cdef_search;
- * clpf_strength[plane] / clpf_log2[plane]: the outcome of clpf_rdo (0 = plane not filtered). */
+ * clpf_strength[plane] / clpf_log2[plane]: the outcome of clpf_rdo (0 = plane not filtered).
+ * clpf_fb_on: the luma per-filter-block decisions, one byte per 2^clpf_log2[0] filter block in raster order (k * blocks per row + l), as the
+ * encoder's clpf_decision callback returned them for (k, l) and as they were signalled; NULL when enable_fb_flag is 0 (every block that is not
+ * all skip is filtered).  Chroma never carries such flags. */
 int tb_filter_frame(tb_filter_ctx *c, yuv_frame_t *rec, const deblock_data_t *deblock_data, int qp, int bitdepth, int cdef_damping, const int8_t *fb_pri[2],
-                    const int8_t *fb_sec[2], const int clpf_strength[3], const int clpf_log2[3], int download) {
+                    const int8_t *fb_sec[2], const int clpf_strength[3], const int clpf_log2[3], const uint8_t *clpf_fb_on, int download) {
   for (int i = 0; i < c->nblk; i++) { /* 364-byte deblock_data_t -> 16 bytes */
     const deblock_data_t *d = &deblock_data[i];
     tb_blkinfo_t *b = &c->bi_host[i];
@@ -59,8 +65,14 @@ int tb_filter_frame(tb_filter_ctx *c, yuv_frame_t *rec, const deblock_data_t *de
   }
   for (int plane = 0; plane < 3 && rc == TB_OK; plane++)
     rc = tb_cdef_frame(c->rec, c->scratch, c->bi_dev, c->fb_pri_dev[plane != 0], c->fb_sec_dev[plane != 0], cdef_damping, cdef_damping, c->dirvar_dev, bitdepth, plane);
+  if (rc == TB_OK && clpf_strength[0] && clpf_fb_on) {
+    const int fb = 1 << clpf_log2[0];
+    rc = tb_memcpy_h2d(c->clpf_fb_on_dev, clpf_fb_on, (size_t)((c->width + fb - 1) / fb) * ((c->height + fb - 1) / fb));
+  }
   for (int plane = 0; plane < 3 && rc == TB_OK; plane++)
-    if (clpf_strength[plane]) rc = tb_clpf_frame(c->rec, c->scratch, c->bi_dev, NULL, clpf_log2[plane], clpf_strength[plane], bitdepth, plane, qp);
+    if (clpf_strength[plane])
+      rc = tb_clpf_frame(c->rec, c->scratch, c->bi_dev, plane == 0 && clpf_fb_on ? c->clpf_fb_on_dev : NULL, clpf_log2[plane], clpf_strength[plane], bitdepth,
+                         plane, qp);
   if (rc == TB_OK) rc = tb_create_reference_frame(c->ref_out, c->rec); /* padded reference stays in HBM for the next frame's searches */
   if (rc == TB_OK && download) rc = tb_frame_download(c->rec, rec->y, rec->stride_y, rec->u, rec->v, rec->stride_c);
   return rc;

@@ -103,12 +103,13 @@ class Frame:
         return f
 
 
-def random_blkinfo(rng, width, height, p_skip=0.3):
-    """A plausible random coding-block partition on the 4x4 grid: returns (numpy BLKINFO [h/4, w/4], DeblockData array)."""
+def random_blkinfo(rng, width, height, p_skip=0.3, root=64, mv_range=9):
+    """A plausible random coding-block partition on the 4x4 grid: returns (numpy BLKINFO [h/4, w/4], DeblockData array).
+    root: the largest coding block (64, or 128 for the encoder's super blocks); motion vectors lie within +-mv_range."""
     bw, bh = width // 4, height // 4
     bi = np.zeros((bh, bw), dtype=BLKINFO)
-    for y0 in range(0, height, 64):
-        for x0 in range(0, width, 64):
+    for y0 in range(0, height, root):
+        for x0 in range(0, width, root):
             def fill(x, y, size):
                 if size > 8 and (rng.random() < 0.5 or x + size > width or y + size > height):
                     h = size // 2
@@ -126,17 +127,22 @@ def random_blkinfo(rng, width, height, p_skip=0.3):
                 rec["tb_split"] = int(rng.integers(0, 2)) if mode != 0 else 0
                 rec["pb_part"] = int(rng.integers(0, 4)) if mode in (2, 3) else 0
                 if mode != 1:
-                    rec["mv0x"], rec["mv0y"] = int(rng.integers(-9, 10)), int(rng.integers(-9, 10))
+                    rec["mv0x"], rec["mv0y"] = int(rng.integers(-mv_range, mv_range + 1)), int(rng.integers(-mv_range, mv_range + 1))
                     if mode == 3:
-                        rec["mv1x"], rec["mv1y"] = int(rng.integers(-9, 10)), int(rng.integers(-9, 10))
+                        rec["mv1x"], rec["mv1y"] = int(rng.integers(-mv_range, mv_range + 1)), int(rng.integers(-mv_range, mv_range + 1))
                 bi[y // 4:min(bh, (y + size) // 4), x // 4:min(bw, (x + size) // 4)] = rec
-            fill(x0, y0, 64)
-    dd = (DeblockData * (bw * bh))()
+            fill(x0, y0, root)
+    return bi, deblock_data(bi)
+
+
+def deblock_data(bi):
+    """the DeblockData array of a BLKINFO grid (the fields the in-loop filters read)"""
     flat = bi.reshape(-1)
-    for i in range(bw * bh):
+    dd = (DeblockData * flat.size)()
+    for i in range(flat.size):
         d, r = dd[i], flat[i]
         d.mode = int(r["mode"]); d.cbp.y = int(r["cbp_y"]); d.size = int(r["size"]); d.tb_split = int(r["tb_split"])
         d.pb_part = int(r["pb_part"])
         d.inter_pred.mv0.x, d.inter_pred.mv0.y = int(r["mv0x"]), int(r["mv0y"])
         d.inter_pred.mv1.x, d.inter_pred.mv1.y = int(r["mv1x"]), int(r["mv1y"])
-    return bi, dd
+    return dd
