@@ -6,8 +6,8 @@
 // simulates warps with threads): every warp executes the whole control flow on its own scratch blocks (Work), so sequential sections
 // (neighbour derivation, the bipred refinement, the recursion itself) are simply replicated and stay consistent without communication.
 // Two kinds of sections are DISTRIBUTED: the motion searches of the reference frames (one reference per warp; results exchanged through
-// the backend and the candidate lists replayed by the other warps) and the RD candidates of a block (round robin in the serial form of the
-// decision, drawn from shared counters in the overlapped form: mode_decision_overlap).  The reference keeps the first candidate with the
+// the backend and the candidate lists replayed by the other warps) and the RD candidates of a block (round robin, or partly drawn from shared
+// counters where mode_decision_rdo overlaps the sections of a decision).  The reference keeps the first candidate with the
 // strictly smallest cost; that is the minimum of (cost, k), k = the candidate's position in the reference's evaluation order, which the
 // backend's reduction returns together with the warp that holds the winning reconstruction; that warp alone commits the block.
 // The backend's primitives are the warp-cooperative routines of tb_device.cuh.  Nothing in this file touches samples directly.
@@ -179,14 +179,14 @@ template <class S, class B> struct Rdo {
   int best_ref;      // frame_info->best_ref (per super block)
   int sb_index;
   int n_leaves, coeff_used;
-  // distributed candidate evaluation: running candidate index and this warp's best so far
-  int cidx, loc_idx;
+  // distributed candidate evaluation: this warp's best (cost, index) so far and the range of its inter costs
+  int loc_idx;
   uint32_t loc_cost, loc_worst, loc_bestc;
   // the candidate about to be evaluated has the same inter prediction as the previous one of this warp (same vectors, another tb_param): W.p_* is still valid
   bool reuse_pred;
 
   TBR_HD Rdo(FrameCtx<S> &f, Work<S> &w, Work<S> &w0, B &b)
-      : F(f), W(w), W0(w0), be(b), best_ref(-1), sb_index(0), n_leaves(0), coeff_used(0), cidx(0), loc_idx(0), loc_cost(MAX_U32), loc_worst(0), loc_bestc(MAX_U32), reuse_pred(false) {}
+      : F(f), W(w), W0(w0), be(b), best_ref(-1), sb_index(0), n_leaves(0), coeff_used(0), loc_idx(0), loc_cost(MAX_U32), loc_worst(0), loc_bestc(MAX_U32), reuse_pred(false) {}
 
   // ---------------------------------------------------------------------------------------------------------------
   // neighbour state
@@ -413,24 +413,10 @@ template <class S, class B> struct Rdo {
       inter_pred_yuv(c.ref_idx0, W.p_y, W.p_u, W.p_v, bi.ypos, bi.xpos, bi.size, bi.bwidth, bi.bheight, c.mv0, F.ref_sign[c.ref_idx0], split);
   }
 
-  // encode_and_reconstruct_block_inter :1275-1338 for one plane (orig/pred/rec compact or strided; coefficients in the reference layout)
-  TBR_HD TBR_NI int enc_rec_inter(const S *orig, int os, int size, int qp, const S *pred, int16_t *cq, S *rec, int coeff_type, int tb_split) {
-    if (tb_split) {
-      const int s2 = size / 2;
-      int cbp = 0, index = 0;
-      for (int i = 0; i < size; i += s2)
-        for (int j = 0; j < size; j += s2) {
-          const int fast = (size == 64 || F.speed > 1) ? 1 : 0;
-          const int bit = be.tx_chain(orig + i * os + j, os, pred + i * size + j, size, rec + i * size + j, size, cq + index, s2, qp, coeff_type, fast);
-          cbp = (cbp << 1) + bit;
-          index += 256;
-        }
-      return cbp;
-    }
-    const int fast = ((size == 64 && F.speed > 0) || F.speed > 1) ? 1 : 0;
-    return be.tx_chain(orig, os, pred, size, rec, size, cq, size, qp, coeff_type, fast);
-  }
-  // the chains of enc_rec_inter for one plane, appended to a job list (same order, same fast flags); returns the number of chains
+  // the fast flag of the inter transform chains of a size x size block (encode_and_reconstruct_block_inter :1275-1338)
+  TBR_HD int inter_fast(int size, int tb_split) const { return tb_split ? size == 64 || F.speed > 1 : (size == 64 && F.speed > 0) || F.speed > 1; }
+  // the transform chains of encode_and_reconstruct_block_inter :1275-1338 for one plane (orig/pred/rec compact or strided; coefficients in the
+  // reference layout), appended to a job list in the reference's order; returns the number of chains
   TBR_HD int inter_jobs(TxJob<S> *jobs, const S *orig, int os, int size, int qp, const S *pred, int16_t *cq, S *rec, int coeff_type, int tb_split) const {
     if (tb_split) {
       const int s2 = size / 2;
@@ -439,15 +425,30 @@ template <class S, class B> struct Rdo {
         for (int j = 0; j < size; j += s2) {
           TxJob<S> &q = jobs[n];
           q.orig = orig + i * os + j; q.os = os; q.pred = pred + i * size + j; q.ps = size; q.rec = rec + i * size + j; q.rs = size; q.cq = cq + 256 * n; q.size = s2; q.qp = qp;
-          q.coeff_type = coeff_type; q.fast = (size == 64 || F.speed > 1) ? 1 : 0;
+          q.coeff_type = coeff_type; q.fast = inter_fast(size, 1);
           n++;
         }
       return 4;
     }
     TxJob<S> &q = jobs[0];
     q.orig = orig; q.os = os; q.pred = pred; q.ps = size; q.rec = rec; q.rs = size; q.cq = cq; q.size = size; q.qp = qp; q.coeff_type = coeff_type;
-    q.fast = ((size == 64 && F.speed > 0) || F.speed > 1) ? 1 : 0;
+    q.fast = inter_fast(size, 0);
     return 1;
+  }
+  // encode_and_reconstruct_block_inter for one plane: the chains of inter_jobs one after the other, without the job list; returns the cbp
+  TBR_HD TBR_NI int enc_rec_inter(const S *orig, int os, int size, int qp, const S *pred, int16_t *cq, S *rec, int coeff_type, int tb_split) {
+    if (tb_split) {
+      const int s2 = size / 2;
+      int cbp = 0, index = 0;
+      for (int i = 0; i < size; i += s2)
+        for (int j = 0; j < size; j += s2) {
+          const int bit = be.tx_chain(orig + i * os + j, os, pred + i * size + j, size, rec + i * size + j, size, cq + index, s2, qp, coeff_type, inter_fast(size, 1));
+          cbp = (cbp << 1) + bit;
+          index += 256;
+        }
+      return cbp;
+    }
+    return be.tx_chain(orig, os, pred, size, rec, size, cq, size, qp, coeff_type, inter_fast(size, 0));
   }
   TBR_HD static int join_cbp(const int *bit, int n) {
     int cbp = 0;
@@ -718,15 +719,28 @@ template <class S, class B> struct Rdo {
   // ---------------------------------------------------------------------------------------------------------------
   // mode_decision_rdo :1835-2120
   // ---------------------------------------------------------------------------------------------------------------
-  TBR_HD void cand_group_begin() { cidx = 0; loc_idx = 0x7fffffff; loc_cost = MAX_U32; loc_worst = 0; loc_bestc = MAX_U32; }
-  // candidate number cidx of the current group: evaluated by the warp that owns it; track_range: also the worst / best cost (:1998-1999)
-  TBR_HD TBR_NI void try_cand(BlockInfo &bi, Cand &c, int w, int h, bool track_range = false) {
-    const int my = cidx++;
-    if (!be.mine(my)) return;
+  // candidate indices in the reference's evaluation order after skip (k) and merge (num_skip + k * max_tb + tb): inter (IDX_INTER + (reference,
+  // partition) * (max_tb + 1) + tb_param + 1), bipred (IDX_BIPRED + tb_param, then the joint search of B frames), intra (IDX_INTRA + tb_param)
+  enum { IDX_INTER = 64, IDX_BIPRED = IDX_INTER + TB_RDO_MAX_REF * 4 * 3, IDX_INTRA = IDX_BIPRED + 8 };
+
+  TBR_HD void cand_group_begin() { loc_idx = 0x7fffffff; loc_cost = MAX_U32; loc_worst = 0; loc_bestc = MAX_U32; }
+  // candidate `idx` evaluated by whichever warp calls this; the warp keeps its best (cost, idx); track_range: also the worst / best cost (:1998-1999)
+  TBR_HD TBR_NI void eval_cand(BlockInfo &bi, Cand &c, int w, int h, int idx, bool track_range) {
     const int nbits = encode_block(bi, c);
     const uint32_t cost = cost_calc(bi, w, h, nbits);
     if (track_range) { loc_worst = loc_worst > cost ? loc_worst : cost; loc_bestc = loc_bestc < cost ? loc_bestc : cost; }
-    if (cost < loc_cost) { loc_cost = cost; loc_idx = my; copy_best(bi, c); }
+    if (cost < loc_cost || (cost == loc_cost && idx < loc_idx)) { loc_cost = cost; loc_idx = idx; copy_best(bi, c); }
+  }
+  // the tb_param variants tb0 .. max_tb - 1 of candidate c, indices idx, idx + 1, ..: dealt round robin by their position in the group (*pos), or,
+  // when the calling warp owns them all (own), evaluated here on one prediction
+  TBR_HD TBR_NI void eval_tbs(BlockInfo &bi, Cand &c, int tb0, int idx, bool own, int *pos, bool track_range) {
+    for (int tb = tb0; tb < bi.max_tb; tb++, idx++, (*pos)++) {
+      if (!own && !be.mine(*pos)) continue;
+      c.tb_param = tb;
+      reuse_pred = own && tb > tb0;
+      eval_cand(bi, c, bi.size, bi.size, idx, track_range);
+    }
+    reuse_pred = false;
   }
   // end of a group: the winner over all warps = min (cost, index); every warp receives its cost and parameters, `owner` holds its blocks
   TBR_HD uint32_t cand_group_end(BlockInfo &bi, int *owner) {
@@ -739,50 +753,81 @@ template <class S, class B> struct Rdo {
   TBR_HD static void set_from_ipred(Cand &c, const IPred &p, int idx) {
     c.skip_idx = idx; c.ref_idx0 = p.ref_idx0; c.ref_idx1 = p.ref_idx1; c.mv0[0] = p.mv0; c.mv1[0] = p.mv1; c.dir = p.bipred_flag;
   }
+  // one item of the intra-mode search (:2080-2097 with intra_rdo, else search_intra_prediction_params): the warp keeps its best (cost, k)
+  TBR_HD TBR_NI void intra_search_item(BlockInfo &bi, Cand &t, int k, uint32_t *best_cost, int *best_k) {
+    if (F.intra_rdo) {
+      t.intra_mode = k / bi.max_tb; t.tb_param = k % bi.max_tb; t.mode = MODE_INTRA;
+      const int nbits = encode_block(bi, t);
+      const uint32_t cost = cost_calc(bi, bi.size, bi.size, nbits);
+      if (cost < *best_cost || (cost == *best_cost && k < *best_k)) { *best_cost = cost; *best_k = k; }
+    } else {
+      int mode;
+      search_intra(bi, &mode);
+      *best_cost = 0; *best_k = mode * bi.max_tb;
+    }
+  }
+  // the bi-prediction candidates (BIPRED_PART = 0: one partition): search_bipred_prediction_params, a chain of dependent searches, and its tb_param
+  // variants; in B frames at encoder_speed 0 also the candidate of the joint search (me_mode 1)
+  TBR_HD TBR_NI void bipred_cands(BlockInfo &bi, Cand &t, const Mv *mv_center, Mv mvp, bool own, int *pos) {
+    search_bipred(bi, 0, mv_center, mvp, &t.ref_idx0, &t.ref_idx1, t.mv0, t.mv1, 0);
+    t.mode = MODE_BIPRED; t.pb_part = PART_NONE;
+    eval_tbs(bi, t, 0, IDX_BIPRED, own, pos, false);
+    if (F.frame_type == B_FRAME && F.speed == 0) {
+      search_bipred(bi, 1, mv_center, mvp, &t.ref_idx0, &t.ref_idx1, t.mv0, t.mv1, 1);
+      t.tb_param = 0;
+      if (own || be.mine(*pos)) eval_cand(bi, t, bi.size, bi.size, IDX_BIPRED + bi.max_tb, false);
+      (*pos)++;
+    }
+    be.mark(PH_BIPRED);
+  }
 
-  TBR_HD TBR_NI uint32_t mode_decision_serial(BlockInfo &bi, int *owner) {
+  // mode_decision_rdo :1835-2120.  The candidates in the reference's order: skip, merge x tb_param, inter (reference x partition x tb_param), bipred,
+  // the joint bipred of B frames, intra x tb_param; the warps deal them round robin by their position in the group.
+  // Square blocks of inter frames at encoder_speed 0 on more than one warp OVERLAP the sections that do not depend on each other instead:
+  //   while the references' motion searches run (one warp per reference), the remaining warps start the intra-mode search;
+  //   then warp 0 runs the bi-prediction chain (every search depends on the previous one) and evaluates its candidates, while the others draw the
+  //   inter candidates (one draw = the tb_param variants of one prediction) and the rest of the intra-mode search from shared counters;
+  //   the candidate lists the chain extends are copied to the other warps' replicas afterwards.
+  // The schedule decides only which warp evaluates what, and when: the winner = min (cost, index) is the reference's "first candidate with the
+  // strictly smallest cost" either way.
+  TBR_HD TBR_NI uint32_t mode_decision_rdo(BlockInfo &bi, int *owner) {
     const int size = bi.size, ypos = bi.ypos, xpos = bi.xpos;
     const int rectangular = bi.bwidth != size || bi.bheight != size;
     const int intra_inter_sad = F.speed > 0;
-    uint32_t sad_intra = MAX_U32;
-    int do_inter = 1, do_intra = 1;
+    const bool overlap = F.frame_type != I_FRAME && F.speed == 0 && !rectangular && size <= MAX_TR && be.nwarps() > 1;
+    const int n_isearch = F.intra_rdo ? F.num_intra_modes * bi.max_tb : 1;  // items of the intra-mode search
+    uint32_t sad_intra = MAX_U32, my_icost = MAX_U32;
+    int do_inter = 1, do_intra = 1, my_ik = 0x7fffffff, pos = 0;
+    if (overlap) { be.queue_reset(); be.mark2(-1); }
+    be.mark(PH_OTHER);
     cand_group_begin();
-    Cand t;
-    t.mode = MODE_SKIP; t.intra_mode = 0; t.skip_idx = 0; t.pb_part = PART_NONE; t.ref_idx0 = t.ref_idx1 = 0; t.dir = 0; t.cbp_y = t.cbp_u = t.cbp_v = 0; t.tb_param = 0; t.tb_split = 0;
-    for (int i = 0; i < 4; i++) { t.mv0[i].x = t.mv0[i].y = t.mv1[i].x = t.mv1[i].y = 0; }
-    int intra_mode = 0;
+    Cand t = {};  // MODE_SKIP, PART_NONE, tb_param 0, zero vectors
 
-    if (F.frame_type != I_FRAME) {
-      t.tb_param = 0; t.pb_part = PART_NONE; t.mode = MODE_SKIP;
-      for (int k = 0; k < bi.num_skip; k++) {
+    if (F.frame_type != I_FRAME)
+      for (int k = 0; k < bi.num_skip; k++, pos++) {
         set_from_ipred(t, bi.skip_cand[k], k);
-        t.mode = MODE_SKIP;
-        try_cand(bi, t, bi.bwidth, bi.bheight);
+        if (be.mine(pos)) eval_cand(bi, t, bi.bwidth, bi.bheight, k, false);
       }
-    }
     if ((size < 128 || F.speed == 0) && !rectangular && size <= MAX_TR) {
       if (F.frame_type != I_FRAME) {
-        t.tb_param = 0;
-        be.mark(PH_OTHER);
+        t.mode = MODE_MERGE;
         for (int k = 0; k < bi.num_merge; k++) {
           set_from_ipred(t, bi.merge_cand[k], k);
-          t.mode = MODE_MERGE;
-          for (int tb = 0; tb <= bi.max_tb - 1; tb++) { t.tb_param = tb; try_cand(bi, t, size, size); }
+          if (!overlap || be.mine(bi.num_skip + k)) eval_tbs(bi, t, 0, bi.num_skip + k * bi.max_tb, overlap, &pos, false);
         }
+        be.mark(PH_SKIP_MERGE);
         if (intra_inter_sad) {
-          sad_intra = (uint32_t)search_intra(bi, &intra_mode);
-          sad_intra += (uint32_t)(int)mul_add_half(F.sqrt_lambda, 2.0);
+          int mode;
+          sad_intra = (uint32_t)search_intra(bi, &mode) + (uint32_t)(int)mul_add_half(F.sqrt_lambda, 2.0);
         }
-        t.mode = MODE_INTER;
-        int min_idx, max_idx;
-        if (best_ref < 0 || F.speed < 2 || F.enable_bipred) { min_idx = 0; max_idx = F.num_ref - 1; }
-        else min_idx = max_idx = best_ref;
+        int min_idx = 0, max_idx = F.num_ref - 1;
+        if (best_ref >= 0 && F.speed >= 2 && !F.enable_bipred) min_idx = max_idx = best_ref;
         if (F.frame_type == B_FRAME && F.interp_ref > 2) min_idx = 1;
-        Mv mv_all[TB_RDO_MAX_REF][4][4], mv_center[TB_RDO_MAX_REF], mvp;
+        const int nrs = max_idx - min_idx + 1;
+        Mv mv_all[TB_RDO_MAX_REF][4][4], mv_center[TB_RDO_MAX_REF];
         uint32_t sad_inter_r[TB_RDO_MAX_REF];
         const S *oy = F.org[0] + ypos * F.org_stride[0] + xpos;
-        be.mark(PH_SKIP_MERGE);
-        mvp = get_mv_pred(ypos, xpos, size, size);  // the same for every reference (its ref_idx argument is unused, inter_prediction.c:413)
+        const Mv mvp = get_mv_pred(ypos, xpos, size, size);  // the same for every reference (its ref_idx argument is unused, inter_prediction.c:413)
         bi.mvp = mvp;
         // (1) the searches: reference ref_idx on warp (ref_idx - min_idx) mod NW.  A reference's searches only read and extend ITS candidate list
         for (int ref_idx = min_idx; ref_idx <= max_idx; ref_idx++) {
@@ -800,7 +845,14 @@ template <class S, class B> struct Rdo {
           sad_inter_r[ref_idx] = sad_inter;
           be.put_me(ref_idx, &mv_all[ref_idx][0][0], sad_inter);
         }
+        if (overlap) {  // the warps without a reference begin the intra-mode search
+          be.mark2(0);
+          if (be.warp() >= nrs)
+            for (int k; (k = be.next(1)) < n_isearch;) intra_search_item(bi, t, k, &my_icost, &my_ik);
+          be.mark2(1);
+        }
         be.cta_sync();
+        if (overlap) be.mark2(2);  // (diagnostics) the wait for the slowest warp of the phase
         // (2) every warp learns the other references' vectors and replays their effect on its replica of the candidate lists
         for (int ref_idx = min_idx; ref_idx <= max_idx; ref_idx++) {
           if (be.mine(ref_idx - min_idx)) continue;
@@ -812,254 +864,56 @@ template <class S, class B> struct Rdo {
         }
         be.cta_sync();
         be.mark(PH_SEARCH);
-        // (3) the RD candidates of every reference
-        for (int ref_idx = min_idx; ref_idx <= max_idx; ref_idx++) {
-          t.ref_idx0 = t.ref_idx1 = ref_idx;
+        // (3) the RD candidates of the references (overlapped: drawn, while warp 0 runs the bi-prediction chain first)
+        const bool do_bipred = F.num_ref > 1 && F.enable_bipred;
+        if (overlap && do_bipred && be.warp() == 0) bipred_cands(bi, t, mv_center, mvp, true, &pos);
+        const int ntb = bi.max_tb + 1, min_tb = F.speed < 1 ? -1 : 0;  // tb_param -1: no residual (:1990)
+        for (int g = overlap ? be.next(0) : 0; g < nrs * bi.max_pb; g = overlap ? be.next(0) : g + 1) {
+          const int part = g % bi.max_pb, ref_idx = min_idx + g / bi.max_pb;
           if (intra_inter_sad) {
             do_inter = sad_inter_r[ref_idx] < sad_intra;
-            if (sad_inter_r[ref_idx] < sad_intra) do_intra = 0;
+            if (do_inter) do_intra = 0;
           }
-          if (do_inter) {
-            for (int part = 0; part < bi.max_pb; part++) {
-              t.pb_part = part;
-              for (int i = 0; i < 4; i++) t.mv0[i] = t.mv1[i] = mv_all[ref_idx][part][i];
-              const int min_tb = F.speed < 1 ? -1 : 0;
-              t.mode = MODE_INTER; t.dir = 0;
-              for (int tb = min_tb; tb <= bi.max_tb - 1; tb++) {
-                t.tb_param = tb;
-                try_cand(bi, t, size, size, true);
-              }
-            }
-          }
+          if (!do_inter) continue;
+          t.mode = MODE_INTER; t.dir = 0; t.ref_idx0 = t.ref_idx1 = ref_idx; t.pb_part = part;
+          for (int i = 0; i < 4; i++) t.mv0[i] = t.mv1[i] = mv_all[ref_idx][part][i];
+          eval_tbs(bi, t, min_tb, IDX_INTER + g * ntb + min_tb + 1, overlap, &pos, true);
+        }
+        be.mark(PH_INTER_CAND);
+        if (overlap) {  // the rest of the intra-mode search
+          for (int k; (k = be.next(1)) < n_isearch;) intra_search_item(bi, t, k, &my_icost, &my_ik);
+          be.mark(PH_INTRA_SEARCH);
         }
         {
           uint32_t worst_cost = loc_worst, best_cost = loc_bestc;
           be.reduce_range(&worst_cost, &best_cost);
           if (worst_cost && (uint64_t)worst_cost * 3 > (uint64_t)best_cost * 4) best_ref = 0;  // best_ref_idx is never updated in the reference (:1868, :2019)
         }
-        be.mark(PH_INTER_CAND);
-
-        if (F.num_ref > 1 && F.enable_bipred && do_inter) {
-          int r0, r1;
-          Mv a0[4], a1[4];
-          // BIPRED_PART = 0: one partition
-          search_bipred(bi, 0, mv_center, mvp, &r0, &r1, a0, a1, 0);
-          t.pb_part = 0; t.ref_idx0 = r0; t.ref_idx1 = r1;
-          for (int i = 0; i < 4; i++) { t.mv0[i] = a0[i]; t.mv1[i] = a1[i]; }
-          t.mode = MODE_BIPRED;
-          for (int tb = 0; tb <= bi.max_tb - 1; tb++) { t.tb_param = tb; try_cand(bi, t, size, size); }
-          if (F.frame_type == B_FRAME && F.speed == 0) {
-            search_bipred(bi, 1, mv_center, mvp, &r0, &r1, a0, a1, 1);
-            t.pb_part = PART_NONE; t.ref_idx0 = r0; t.ref_idx1 = r1;
-            for (int i = 0; i < 4; i++) { t.mv0[i] = a0[i]; t.mv1[i] = a1[i]; }
-            t.tb_param = 0; t.mode = MODE_BIPRED;
-            try_cand(bi, t, size, size);
-          }
-        }
-      }
-      be.mark(PH_BIPRED);
-      if (do_intra) {
-        t.mode = MODE_INTRA;
-        if (F.intra_rdo) {
-          // choice of the intra mode by RD cost (:2080-2097): its own distributed group, no copy_best
-          uint32_t min_intra_cost = MAX_U32;
-          int best_k = 0x7fffffff, k = 0;
-          for (int m = 0; m < F.num_intra_modes; m++) {
-            t.intra_mode = m;
-            for (int tb = 0; tb <= bi.max_tb - 1; tb++, k++) {
-              if (!be.mine(k)) continue;
-              t.tb_param = tb; t.mode = MODE_INTRA;
-              const int nbits = encode_block(bi, t);
-              const uint32_t cost = cost_calc(bi, size, size, nbits);
-              if (cost < min_intra_cost) { min_intra_cost = cost; best_k = k; }
+        if (!overlap && do_bipred && do_inter) bipred_cands(bi, t, mv_center, mvp, false, &pos);
+        if (overlap && do_bipred) {  // warp 0's searches extended (and scribbled on, :873-881) the candidate lists: everybody's replica follows
+          if (be.warp() != 0)
+            for (int r = 0; r < F.num_ref; r++) {
+              be.copy_words(W.mvcand[r], W0.mvcand[r], 64 * (int)sizeof(Mv) / 4);
+              W.mvcand_num[r] = W0.mvcand_num[r]; W.mvcand_mask[r] = W0.mvcand_mask[r];
             }
-          }
-          be.reduce_best(&min_intra_cost, &best_k);
-          intra_mode = min_intra_cost == MAX_U32 ? 0 : best_k / bi.max_tb;
-        } else
-          search_intra(bi, &intra_mode);
-        t.intra_mode = intra_mode;
-        be.mark(PH_INTRA_SEARCH);
-        for (int tb = 0; tb <= bi.max_tb - 1; tb++) { t.tb_param = tb; t.mode = MODE_INTRA; try_cand(bi, t, size, size); }
-      }
-    }
-    const uint32_t cost_ = cand_group_end(bi, owner);
-    be.mark(PH_INTRA_CAND);
-    return cost_;
-  }
-
-
-  // candidate `idx` (its position in the reference's evaluation order) evaluated by whichever warp calls this; the warp keeps its best (cost, idx)
-  TBR_HD TBR_NI void eval_cand(BlockInfo &bi, Cand &c, int w, int h, int idx, bool track_range) {
-    const int nbits = encode_block(bi, c);
-    const uint32_t cost = cost_calc(bi, w, h, nbits);
-    if (track_range) { loc_worst = loc_worst > cost ? loc_worst : cost; loc_bestc = loc_bestc < cost ? loc_bestc : cost; }
-    if (cost < loc_cost || (cost == loc_cost && idx < loc_idx)) { loc_cost = cost; loc_idx = idx; copy_best(bi, c); }
-  }
-  // one item of the intra-mode search (:2080-2097 with intra_rdo, else search_intra_prediction_params): the warp keeps its best (cost, k)
-  TBR_HD TBR_NI void intra_search_item(BlockInfo &bi, Cand &t, int k, uint32_t *best_cost, int *best_k) {
-    if (F.intra_rdo) {
-      t.intra_mode = k / bi.max_tb; t.tb_param = k % bi.max_tb; t.mode = MODE_INTRA;
-      const int nbits = encode_block(bi, t);
-      const uint32_t cost = cost_calc(bi, bi.size, bi.size, nbits);
-      if (cost < *best_cost || (cost == *best_cost && k < *best_k)) { *best_cost = cost; *best_k = k; }
-    } else {
-      int mode;
-      search_intra(bi, &mode);
-      *best_cost = 0; *best_k = mode * bi.max_tb;
-    }
-  }
-
-  // mode_decision_rdo for square blocks of inter frames at encoder_speed 0, with the sections of the decision that do not depend on each other
-  // OVERLAPPED over the warps of the CTA instead of run one after the other:
-  //   while the references' motion searches run (one warp per reference), the remaining warps start the intra-mode search;
-  //   then ONE warp runs the bi-prediction chain (search_bipred_prediction_params: every search depends on the previous one) and evaluates its
-  //   candidates, while the others draw the inter candidates and the rest of the intra-mode search from shared counters.
-  // Every candidate keeps the index it has in the reference's evaluation order, so the winner = min (cost, index) is the reference's
-  // "first candidate with the strictly smallest cost" whichever warp evaluated what.  The candidate lists the chain extends are copied to
-  // the other warps' replicas afterwards.
-  TBR_HD TBR_NI uint32_t mode_decision_overlap(BlockInfo &bi, int *owner) {
-    const int size = bi.size, ypos = bi.ypos, xpos = bi.xpos, nw = be.nwarps();
-    be.queue_reset();
-    be.mark2(-1);
-    cand_group_begin();
-    Cand t;
-    t.mode = MODE_SKIP; t.intra_mode = 0; t.skip_idx = 0; t.pb_part = PART_NONE; t.ref_idx0 = t.ref_idx1 = 0; t.dir = 0; t.cbp_y = t.cbp_u = t.cbp_v = 0; t.tb_param = 0; t.tb_split = 0;
-    for (int i = 0; i < 4; i++) { t.mv0[i].x = t.mv0[i].y = t.mv1[i].x = t.mv1[i].y = 0; }
-    be.mark(PH_OTHER);
-    int idx = 0;
-    for (int k = 0; k < bi.num_skip; k++, idx++) {
-      if (!be.mine(idx)) continue;
-      set_from_ipred(t, bi.skip_cand[k], k);
-      t.mode = MODE_SKIP; t.tb_param = 0; t.pb_part = PART_NONE;
-      eval_cand(bi, t, bi.bwidth, bi.bheight, idx, false);
-    }
-    for (int k = 0; k < bi.num_merge; k++) {  // the tb_param variants of one merge candidate share its prediction: same warp
-      const bool my = be.mine(bi.num_skip + k);
-      for (int tb = 0; tb <= bi.max_tb - 1; tb++, idx++) {
-        if (!my) continue;
-        set_from_ipred(t, bi.merge_cand[k], k);
-        t.mode = MODE_MERGE; t.tb_param = tb; t.pb_part = PART_NONE;
-        reuse_pred = tb > 0;
-        eval_cand(bi, t, size, size, idx, false);
-      }
-      reuse_pred = false;
-    }
-    be.mark(PH_SKIP_MERGE);
-
-    int min_idx = 0;
-    const int max_idx = F.num_ref - 1;
-    if (F.frame_type == B_FRAME && F.interp_ref > 2) min_idx = 1;
-    const int nrs = max_idx - min_idx + 1;
-    Mv mv_all[TB_RDO_MAX_REF][4][4], mv_center[TB_RDO_MAX_REF], mvp;
-    uint32_t sad_inter_r[TB_RDO_MAX_REF];
-    const S *oy = F.org[0] + ypos * F.org_stride[0] + xpos;
-    mvp = get_mv_pred(ypos, xpos, size, size);
-    bi.mvp = mvp;
-    const int n_isearch = F.intra_rdo ? F.num_intra_modes * bi.max_tb : 1;
-    uint32_t my_icost = MAX_U32;
-    int my_ik = 0x7fffffff;
-    // (1) the searches, one reference per warp; warps without a reference begin the intra-mode search
-    for (int ref_idx = min_idx; ref_idx <= max_idx; ref_idx++) {
-      if (!be.mine(ref_idx - min_idx)) continue;
-      add_mvcandidate(mvp, ref_idx);
-      const int sign = F.ref_sign[ref_idx];
-      mv_center[ref_idx] = mvp;
-      uint32_t sad_inter = MAX_U32;
-      for (int part = 0; part < bi.max_pb; part++) {
-        const uint32_t sad = (uint32_t)search_inter(oy, F.org_stride[0], ref_idx, bi, mv_center[ref_idx], mvp, mv_all[ref_idx][part], part, sign, ref_idx);
-        for (int i = 0; i < 4; i++) add_mvcandidate(mv_all[ref_idx][part][i], ref_idx);
-        mv_center[ref_idx] = mv_all[ref_idx][0][0];
-        sad_inter = sad_inter < sad ? sad_inter : sad;
-      }
-      sad_inter_r[ref_idx] = sad_inter;
-      be.put_me(ref_idx, &mv_all[ref_idx][0][0], sad_inter);
-    }
-    be.mark2(0);  // (diagnostics) own searches done
-    if (be.warp() >= nrs)
-      for (int k; (k = be.next(1)) < n_isearch;) intra_search_item(bi, t, k, &my_icost, &my_ik);
-    be.mark2(1);  // intra items taken while the searches run
-    be.cta_sync();
-    be.mark2(2);  // wait for the slowest warp of the phase
-    for (int ref_idx = min_idx; ref_idx <= max_idx; ref_idx++) {
-      if (be.mine(ref_idx - min_idx)) continue;
-      be.get_me(ref_idx, &mv_all[ref_idx][0][0], &sad_inter_r[ref_idx]);
-      add_mvcandidate(mvp, ref_idx);
-      for (int part = 0; part < bi.max_pb; part++)
-        for (int i = 0; i < 4; i++) add_mvcandidate(mv_all[ref_idx][part][i], ref_idx);
-      mv_center[ref_idx] = mv_all[ref_idx][0][0];
-    }
-    be.cta_sync();
-    be.mark(PH_SEARCH);
-
-    // (2) the bi-prediction chain on warp 0; inter candidates and the intra-mode search on everybody (warp 0 joins when its chain is done)
-    const int ntb = bi.max_tb + 1;  // tb_param -1 (no residual), 0, .. max_tb - 1 (encoder_speed < 1, :1990)
-    const int n_inter = nrs * bi.max_pb * ntb;
-    const int IDX_INTER = 64, IDX_BIPRED = IDX_INTER + n_inter, IDX_INTRA = IDX_BIPRED + 8;
-    const bool do_bipred = F.num_ref > 1 && F.enable_bipred;
-    if (do_bipred && be.warp() == 0) {
-      int r0, r1;
-      Mv a0[4], a1[4];
-      search_bipred(bi, 0, mv_center, mvp, &r0, &r1, a0, a1, 0);
-      t.pb_part = 0; t.ref_idx0 = r0; t.ref_idx1 = r1; t.dir = 0;
-      for (int i = 0; i < 4; i++) { t.mv0[i] = a0[i]; t.mv1[i] = a1[i]; }
-      t.mode = MODE_BIPRED;
-      for (int tb = 0; tb <= bi.max_tb - 1; tb++) { t.tb_param = tb; reuse_pred = tb > 0; eval_cand(bi, t, size, size, IDX_BIPRED + tb, false); }
-      reuse_pred = false;
-      if (F.frame_type == B_FRAME) {
-        search_bipred(bi, 1, mv_center, mvp, &r0, &r1, a0, a1, 1);
-        t.pb_part = PART_NONE; t.ref_idx0 = r0; t.ref_idx1 = r1;
-        for (int i = 0; i < 4; i++) { t.mv0[i] = a0[i]; t.mv1[i] = a1[i]; }
-        t.tb_param = 0; t.mode = MODE_BIPRED;
-        eval_cand(bi, t, size, size, IDX_BIPRED + bi.max_tb, false);
-      }
-      be.mark(PH_BIPRED);
-    }
-    for (int g; (g = be.next(0)) < nrs * bi.max_pb;) {  // one draw = the tb_param variants of one (reference, partition): they share the prediction
-      const int part = g % bi.max_pb, ref_idx = min_idx + g / bi.max_pb;
-      t.ref_idx0 = t.ref_idx1 = ref_idx; t.pb_part = part;
-      for (int i = 0; i < 4; i++) t.mv0[i] = t.mv1[i] = mv_all[ref_idx][part][i];
-      t.mode = MODE_INTER; t.dir = 0;
-      for (int v = 0; v < ntb; v++) {
-        t.tb_param = v - 1;
-        reuse_pred = v > 0;
-        eval_cand(bi, t, size, size, IDX_INTER + g * ntb + v, true);
-      }
-      reuse_pred = false;
-    }
-    be.mark(PH_INTER_CAND);
-    for (int k; (k = be.next(1)) < n_isearch;) intra_search_item(bi, t, k, &my_icost, &my_ik);
-    be.mark(PH_INTRA_SEARCH);
-    {
-      uint32_t worst_cost = loc_worst, best_cost = loc_bestc;
-      be.reduce_range(&worst_cost, &best_cost);
-      if (worst_cost && (uint64_t)worst_cost * 3 > (uint64_t)best_cost * 4) best_ref = 0;
-    }
-    if (do_bipred) {  // warp 0's searches extended (and scribbled on, :873-881) the candidate lists: everybody's replica follows
-      if (be.warp() != 0)
-        for (int r = 0; r < F.num_ref; r++) {
-          be.copy_words(W.mvcand[r], W0.mvcand[r], 64 * (int)sizeof(Mv) / 4);
-          W.mvcand_num[r] = W0.mvcand_num[r]; W.mvcand_mask[r] = W0.mvcand_mask[r];
+          be.cta_sync();
         }
-      be.cta_sync();
+      }
+      if (do_intra) {
+        if (!overlap) {
+          for (int k = 0; k < n_isearch; k++)
+            if (be.mine(k)) intra_search_item(bi, t, k, &my_icost, &my_ik);
+          be.mark(PH_INTRA_SEARCH);
+        }
+        be.reduce_best(&my_icost, &my_ik);
+        t.mode = MODE_INTRA; t.intra_mode = my_icost == MAX_U32 ? 0 : my_ik / bi.max_tb;
+        if (overlap) pos = 0;  // the overlapped schedule deals only the intra candidates by position
+        eval_tbs(bi, t, 0, IDX_INTRA, false, &pos, false);
+      }
     }
-    be.reduce_best(&my_icost, &my_ik);
-    const int intra_mode = my_icost == MAX_U32 ? 0 : my_ik / bi.max_tb;
-    t.intra_mode = intra_mode;
-    for (int tb = 0; tb <= bi.max_tb - 1; tb++) {
-      if (!be.mine(tb)) continue;
-      t.tb_param = tb; t.mode = MODE_INTRA;
-      eval_cand(bi, t, size, size, IDX_INTRA + tb, false);
-    }
-    const uint32_t cost_ = cand_group_end(bi, owner);
+    const uint32_t cost = cand_group_end(bi, owner);
     be.mark(PH_INTRA_CAND);
-    return cost_;
-  }
-
-  TBR_HD uint32_t mode_decision_rdo(BlockInfo &bi, int *owner) {
-    if (F.frame_type != I_FRAME && F.speed == 0 && bi.bwidth == bi.size && bi.bheight == bi.size && bi.size <= MAX_TR && be.nwarps() > 1)
-      return mode_decision_overlap(bi, owner);
-    return mode_decision_serial(bi, owner);
+    return cost;
   }
 
   // ---------------------------------------------------------------------------------------------------------------
@@ -1101,18 +955,11 @@ template <class S, class B> struct Rdo {
   // :2352-2392.  Skip candidate k (its early-skip test and, if it passes, its RD cost) on warp k mod NW
   TBR_HD TBR_NI int search_early_skip(BlockInfo &bi, uint32_t *cost, int *owner) {
     int flag = 0;
-    Cand t;
-    t.intra_mode = 0; t.pb_part = PART_NONE; t.cbp_y = t.cbp_u = t.cbp_v = 0; t.tb_split = 0;
-    for (int i = 0; i < 4; i++) { t.mv0[i].x = t.mv0[i].y = t.mv1[i].x = t.mv1[i].y = 0; }
+    Cand t = {};  // MODE_SKIP, PART_NONE, tb_param 0, zero vectors
     cand_group_begin();
     for (int k = 0; k < bi.num_skip; k++) {
-      t.tb_param = 0;
       set_from_ipred(t, bi.skip_cand[k], k);
-      t.mode = MODE_SKIP;
-      if (be.mine(cidx)) {
-        if (check_early_skip_block(bi, t)) { flag = 1; try_cand(bi, t, bi.size, bi.size); }
-        else cidx++;
-      } else cidx++;
+      if (be.mine(k) && check_early_skip_block(bi, t)) { flag = 1; eval_cand(bi, t, bi.size, bi.size, k, false); }
     }
     flag = be.reduce_or(flag);
     // the reference encodes the chosen candidate once more (final_encode = 3) and returns that cost: same bits, same reconstruction, same cost
