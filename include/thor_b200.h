@@ -332,8 +332,10 @@ static inline int tb_rdo_coeff_count(int size, int tb_split) {
 }
 
 /* ---- single-block, HOST-buffer forms of host-object functions on the path (staged per call like the drop-in symbols) */
-int tb_quantize(const int16_t *coeff, int16_t *coeffq, int qp, int size, int coeff_block_type); /* quantize(), enc/encode_block.c:84; returns cbp */
-void tb_dequantize(const int16_t *coeffq, int16_t *rcoeff, int qp, int size);                   /* dequantize(), common/common_block.c:45 */
+/* quantize(), enc/encode_block.c:84; returns cbp.  qp must be 0..51 (MAX_QP); any other qp returns TB_ERR_ARG and writes nothing */
+int tb_quantize(const int16_t *coeff, int16_t *coeffq, int qp, int size, int coeff_block_type);
+/* dequantize(), common/common_block.c:45.  qp must be 0..51 (MAX_QP); any other qp sets tb_last_error() and writes nothing */
+void tb_dequantize(const int16_t *coeffq, int16_t *rcoeff, int qp, int size);
 void tb_improve_uv_prediction(int sample_bytes, const void *y, void *u, void *v, const void *ry, int n, int cstride, int stride, int sub,
                               int bitdepth);                                                    /* improve_uv_prediction(), common/common_block.c:347 */
 

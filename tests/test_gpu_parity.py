@@ -96,6 +96,8 @@ def test_dropin_transform_quant(tb, bd):
     L = tb.lib
     lim = (1 << bd) - 1
     for size in (4, 8, 16, 32, 64, 128):
+        q = min(size, 16)
+        coefs = []
         for fast in (0, 1):
             for amp in (lim, 25, 3):
                 blk = aligned((size, size), np.int16)
@@ -103,25 +105,38 @@ def test_dropin_transform_quant(tb, bd):
                 c0 = aligned((size, size), np.int16, fill=0); c1 = aligned((size, size), np.int16, fill=0)
                 O.orc_transform(P(blk), P(c0), size, fast, bd)
                 L.transform_simd(P(blk), P(c1), size, fast, bd)
-                q = min(size, 16)
                 assert (c0[:q, :q] == c1[:q, :q]).all(), (size, fast, amp)
-                for qp in (12, 27, 32, 39, 51):
-                    for typ in (0, 2):
-                        q0 = aligned((q * q,), np.int16, fill=0); q1 = aligned((q * q,), np.int16, fill=0)
-                        cb0 = O.orc_quantize(P(c0), P(q0), qp, size, typ, None)
-                        cb1 = L.tb_quantize(P(c0), P(q1), qp, size, typ)
-                        assert cb0 == cb1 and (q0 == q1).all(), (size, qp, typ, amp)
-                    r0 = aligned((size, size), np.int16, fill=0); r1 = aligned((size, size), np.int16, fill=0)
-                    O.orc_dequantize(P(q0), P(r0), qp, size, None)
-                    L.tb_dequantize(P(q1), P(r1), qp, size)
-                    assert (r0 == r1).all()
-                    if size <= 32:
-                        assert O.orc_check_nz_area(P(r0), size) == L.check_nz_area(P(r0), size)
-                    b0 = aligned((size, size), np.int16, fill=0); b1 = aligned((size, size), np.int16, fill=0)
-                    O.orc_inverse_transform(P(r0), P(b0), size, bd)
-                    if size < 64:  # the reference routes 64/128 through inverse_transform() in transform.c (32x32 kernel + replication)
-                        L.inverse_transform_simd(P(r0), P(b1), size, bd)
-                        assert (b0 == b1).all(), (size, qp)
+                coefs.append((c0, (fast, amp)))
+        # coefficients of magnitude 32768 (and 32767): the bound the quantiser's and dequantiser's 32-bit arithmetic relies on
+        edge = aligned((size, size), np.int16, fill=0)
+        edge[:q, :q] = rng.choice(np.array([-32768, 32767], np.int16), (q, q))
+        coefs.append((edge, "edge"))
+        for c0, what in coefs:
+            for qp in range(52):
+                for typ in range(4):
+                    q0 = aligned((q * q,), np.int16, fill=0); q1 = aligned((q * q,), np.int16, fill=0)
+                    cb0 = O.orc_quantize(P(c0), P(q0), qp, size, typ, None)
+                    cb1 = L.tb_quantize(P(c0), P(q1), qp, size, typ)
+                    assert cb0 == cb1 and (q0 == q1).all(), (size, qp, typ, what)
+                r0 = aligned((size, size), np.int16, fill=0); r1 = aligned((size, size), np.int16, fill=0)
+                O.orc_dequantize(P(q0), P(r0), qp, size, None)
+                L.tb_dequantize(P(q1), P(r1), qp, size)
+                assert (r0 == r1).all(), (size, qp, what)
+                if size <= 32:
+                    assert O.orc_check_nz_area(P(r0), size) == L.check_nz_area(P(r0), size)
+                b0 = aligned((size, size), np.int16, fill=0); b1 = aligned((size, size), np.int16, fill=0)
+                O.orc_inverse_transform(P(r0), P(b0), size, bd)
+                if size < 64:  # the reference routes 64/128 through inverse_transform() in transform.c (32x32 kernel + replication)
+                    L.inverse_transform_simd(P(r0), P(b1), size, bd)
+                    assert (b0 == b1).all(), (size, qp, what)
+        # the edge block itself as levels: the dequantiser's largest products and shifts
+        lv = np.ascontiguousarray(edge[:q, :q]).reshape(-1)
+        for qp in range(52):
+            r0 = aligned((size, size), np.int16, fill=0); r1 = aligned((size, size), np.int16, fill=0)
+            O.orc_dequantize(P(lv), P(r0), qp, size, None)
+            L.tb_dequantize(P(lv), P(r1), qp, size)
+            assert (r0 == r1).all(), (size, qp, "edge levels")
+        assert L.tb_quantize(P(edge), P(q1), 52, size, 0) == tb.TB_ERR_ARG
     for size in (4, 8, 16):
         for _ in range(60):
             blk = aligned((size, size), np.int16)
@@ -470,7 +485,7 @@ def test_batch_txfm_chain(tb, hbd, bd):
         size = sizes[i % 6] if i % 12 < 11 else 4
         x = 4 * int(rng.integers(0, (w - size) // 4 + 1)); y = 4 * int(rng.integers(0, (h - size) // 4 + 1))
         px, py = x + int(rng.integers(-4, 5)), y + int(rng.integers(-4, 5))
-        qp = int(rng.choice([10, 22, 30, 32, 37, 44, 51])); typ = int(rng.integers(0, 4)); fast = int(rng.integers(0, 2))
+        qp = int(rng.integers(0, 52)); typ = int(rng.integers(0, 4)); fast = int(rng.integers(0, 2))
         bits_flag = tb.TXFM_BITS if i % 5 else 0  # most items also ask for the write_coeff bit count (SURVEY 8f.2)
         items[i] = (optr + (y * ost + x) * esz, pptr + (py * pst + px) * esz, recbuf.ptr + recofs * esz, cqbuf.ptr + i * 512, ost, pst, size, size, qp, typ, fast | bits_flag)
         meta.append((size, x, y, px, py, qp, typ, fast, recofs))

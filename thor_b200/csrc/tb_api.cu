@@ -851,6 +851,7 @@ void cdef_filter_block_simd(uint8_t *dst8, uint16_t *dst16, int dstride, const u
 // single-block, host-buffer forms of host-object functions on the path (not reference exports; used by parity tests
 // and by hosts that have not been batched yet)
 int tb_quantize(const int16_t *coeff, int16_t *coeffq, int qp, int size, int coeff_block_type) { /* enc/encode_block.c:84 */
+  if (qp < 0 || qp > 51) { set_err("tb_quantize: qp must be 0..51", cudaSuccess); return TB_ERR_ARG; }  // the device quantiser's 32-bit bound
   need_ctx("quantize");
   const int q = size < 16 ? size : 16;
   int16_t *din = (int16_t *)slot_buf(3, (size_t)size * size * 2), *dout = (int16_t *)slot_buf(2, 512 + 16);
@@ -860,6 +861,7 @@ int tb_quantize(const int16_t *coeff, int16_t *coeffq, int qp, int size, int coe
   return fetch<int32_t>(dout + 256);
 }
 void tb_dequantize(const int16_t *coeffq, int16_t *rcoeff, int qp, int size) { /* common/common_block.c:45 */
+  if (qp < 0 || qp > 51) { set_err("tb_dequantize: qp must be 0..51", cudaSuccess); return; }
   need_ctx("dequantize");
   const int q = size < 16 ? size : 16;
   int16_t *din = (int16_t *)slot_buf(3, 512), *dout = (int16_t *)slot_buf(2, (size_t)size * size * 2);

@@ -1350,6 +1350,76 @@ __device__ __forceinline__ void dot16_block(const int8_t *A, int sa, const int16
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// a10-a13: the arithmetic rules of the transform chain.  Every chain form (the warp_* routines below, thread_txfm4,
+// thread_txfm8, tx_big_chain, DevBackend::tx_multi) keeps its own data movement and takes its stage rounding, scan
+// order, quantiser and dequantiser from here.
+// ---------------------------------------------------------------------------------------------------------------
+__constant__ uint16_t c_quant[6] = {26214, 23302, 20560, 18396, 16384, 14564};  // common/common_tables.c:72
+__constant__ uint16_t c_dequant[6] = {40, 45, 51, 57, 64, 72};                  // common/common_tables.c:73
+
+// scan index of raster position (r,c) in an n x n zig-zag (common/common_tables.c:29-62), closed form
+__host__ __device__ constexpr int zigzag_index(int r, int c, int n) {
+  const int d = r + c;
+  const int before = d < n ? d * (d + 1) / 2 : n * n - (2 * n - 1 - d) * (2 * n - d) / 2;  // samples on earlier diagonals
+  const int lo = d < n ? 0 : d - (n - 1);  // smallest row index on this diagonal
+  // odd diagonals run top-right -> bottom-left (row ascending), even ones the other way
+  const int k = (d & 1) ? (r - lo) : ((d < n ? d : n - 1) - r);
+  return before + k;
+}
+// the same as a table: pos[raster position] = scan index
+template <int N> struct ZigZag {
+  uint8_t pos[N * N];
+  __host__ __device__ constexpr ZigZag() : pos() {
+    for (int p = 0; p < N * N; p++) pos[p] = (uint8_t)zigzag_index(p / N, p % N, N);
+  }
+};
+
+// Rounding of the DCT stages (common/transform.c:245-308, 411-465).  Forward: the first dimension drops log2 size + log2 box-sum
+// scale + bitdepth - 8 bits, the second log2 core size + 5 (core = size / scale); both keep the low 16 bits.  Inverse: the first
+// dimension drops 7 bits, the second 20 - bitdepth; both saturate to int16.  Each stage rounds to nearest (adds half a step).
+struct FwdRound {
+  int shift1, add1, shift2, add2;
+  __device__ __forceinline__ FwdRound(int log2size, int log2scale, int bitdepth)
+      : shift1(log2size + log2scale + bitdepth - 8), add1(1 << (shift1 - 1)), shift2(log2size - log2scale + 5), add2(1 << (shift2 - 1)) {}
+  __device__ __forceinline__ int stage1(int sum) const { return (int16_t)((sum + add1) >> shift1); }
+  __device__ __forceinline__ int stage2(int sum) const { return (int16_t)((sum + add2) >> shift2); }
+};
+struct InvRound {
+  int shift2, add2;
+  __device__ __forceinline__ explicit InvRound(int bitdepth) : shift2(20 - bitdepth), add2(1 << (shift2 - 1)) {}
+  __device__ __forceinline__ static int stage1(int sum) { return iclip((sum + 64) >> 7, -32768, 32767); }
+  __device__ __forceinline__ int stage2(int sum) const { return iclip((sum + add2) >> shift2, -32768, 32767); }
+};
+
+// Quantiser of one transform block (enc/encode_block.c:84-160, no weight matrix), applied along the zig-zag scan: last_pos is the
+// highest position for which last_nz() holds, and the positions up to it are quantised with level(), the level_mode starting at 1
+// and moving by next_mode().  32-bit arithmetic is exact because qp is 0..51: shift2 = 21 - log2 size + qp / 6 <= 27, so
+// |coefficient| * scale + offset <= 32768 * 26214 + (115 << 19) < 2^31.  tb_quantize and the RD loop's check_desc reject other qp.
+struct Quantizer {
+  int scale, shift2, off_last, off0, off1;  // offsets are in 1/256 of a quantiser step
+  __device__ __forceinline__ Quantizer(int qp, int log2size, int coeff_type)  // coeff_type bit 1: intra
+      : scale(c_quant[qp % 6]), shift2(21 - log2size + qp / 6), off_last(((coeff_type & 2) ? 38 : -26) * (1 << (shift2 - 8))),
+        off0(((coeff_type & 2) ? 102 : 51) << (shift2 - 8)), off1(((coeff_type & 2) ? 115 : 90) << (shift2 - 8)) {}
+  __device__ __forceinline__ bool last_nz(int c) const { return (iabs(scale * iabs(c) + off_last) >> shift2) != 0; }
+  // magnitude of the level of coefficient c, entered in level_mode `mode`
+  __device__ __forceinline__ int level(int c, int mode) const {
+    const int ac = scale * iabs(c);
+    return (ac + ((ac >> shift2) > 1 - mode ? off1 : off0)) >> shift2;
+  }
+  __device__ __forceinline__ static int next_mode(int mode, int level) { return mode ? level != 0 : level > 1; }
+};
+
+// Dequantiser (common/common_block.c:45-73, no weight matrix): level * scale, shifted left by qp / 6 - (log2 size - 1), or right
+// with rounding when that is negative, truncated to int16.  |level| <= 32768 and scale <= 72 keep the product below 2^22 and the
+// left shift (at most 7) below 2^29, so 32 bits are exact; the shift is on unsigned so that it is defined for negative levels.
+struct Dequantizer {
+  int scale, lshift, rshift, add;
+  __device__ __forceinline__ Dequantizer(int qp, int log2size)
+      : scale(c_dequant[qp % 6]), lshift(max(qp / 6 - (log2size - 1), 0)), rshift(max(log2size - 1 - qp / 6, 0)), add((1 << rshift) >> 1) {}
+  __device__ __forceinline__ int operator()(int level) const { return (int16_t)(((int)((unsigned)(level * scale) << lshift) + add) >> rshift); }
+};
+
 // per-warp scratch: in[32*33] + tmp[16*33] int16 (padded pitch 33 -> conflict-free column access)
 struct alignas(16) TxScratch {
   alignas(16) int16_t in[48 * 40];   // forward input tile (<= 32 rows, pitch 40) / inverse: rcoeff^T (16 rows) + T^T (32 rows)
@@ -1380,23 +1450,22 @@ __device__ void warp_fwd_transform(const int16_t *block, int bpitch, int size, i
     sc.in[i * 33 + j] = (int16_t)v;
   }
   __syncwarp();
-  const int shift1 = ilog2(size) + ilog2(scale) + bitdepth - 8, add1 = 1 << (shift1 - 1);
-  const int shift2 = l1 + 5, add2 = 1 << (shift2 - 1);
-  // 1st dimension: tmp[i][j] = (sum_k M[i][k] * in[j][k] + add1) >> shift1, i < qsize, j < size1
+  const FwdRound R(ilog2(size), ilog2(scale), bitdepth);
+  // 1st dimension: tmp[i][j] = stage1(sum_k M[i][k] * in[j][k]), i < qsize, j < size1
   for (int p = lane; p < qsize * size1; p += 32) {
     int i = p >> l1, j = p & (size1 - 1);
     int sum = 0;
     for (int k = 0; k < size1; k++) sum += (int)M[(i << l1) + k] * (int)sc.in[j * 33 + k];
-    sc.tmp[i * 33 + j] = (int16_t)((sum + add1) >> shift1);
+    sc.tmp[i * 33 + j] = (int16_t)R.stage1(sum);
   }
   __syncwarp();
-  // 2nd dimension: coef[i][j] = (sum_k M[i][k] * tmp[j][k] + add2) >> shift2, i, j < qsize
+  // 2nd dimension: coef[i][j] = stage2(sum_k M[i][k] * tmp[j][k]), i, j < qsize
   const int lq = ilog2(qsize);
   for (int p = lane; p < qsize * qsize; p += 32) {
     int i = p >> lq, j = p & (qsize - 1);
     int sum = 0;
     for (int k = 0; k < size1; k++) sum += (int)M[(i << l1) + k] * (int)sc.tmp[j * 33 + k];
-    coef[i * qsize + j] = (int16_t)((sum + add2) >> shift2);
+    coef[i * qsize + j] = (int16_t)R.stage2(sum);
   }
   __syncwarp();
 }
@@ -1406,22 +1475,22 @@ __device__ void warp_fwd_transform(const int16_t *block, int bpitch, int size, i
 __device__ void warp_inv_transform(const int16_t *coef, int cpitch, int size, int bitdepth, TxScratch &sc, int16_t *block, int bpitch, const int16_t *tab) {
   const int lane = lane_id();
   const int core = min(size, 32), rep = size / core, lc = ilog2(core), qsize = min(size, 16);
-  const int shift2 = 20 - bitdepth, add2 = 1 << (shift2 - 1);
+  const InvRound R(bitdepth);
   const int16_t *M = tab + dct_tab_ofs(lc);
-  // 1st dimension: tmp[i][j] = clip16((sum_k M[k][j] * coef[k][i] + 64) >> 7), i < qsize, j < core
+  // 1st dimension: tmp[i][j] = stage1(sum_k M[k][j] * coef[k][i]), i < qsize, j < core
   for (int p = lane; p < qsize * core; p += 32) {
     int i = p >> lc, j = p & (core - 1);
     int sum = 0;
     for (int k = 0; k < qsize; k++) sum += (int)M[(k << lc) + j] * (int)coef[k * cpitch + i];
-    sc.tmp[i * 33 + j] = (int16_t)iclip((sum + 64) >> 7, -32768, 32767);
+    sc.tmp[i * 33 + j] = (int16_t)R.stage1(sum);
   }
   __syncwarp();
-  // 2nd dimension: out[i][j] = clip16((sum_k M[k][j] * tmp[k][i] + add2) >> shift2), i, j < core
+  // 2nd dimension: out[i][j] = stage2(sum_k M[k][j] * tmp[k][i]), i, j < core
   for (int p = lane; p < core * core; p += 32) {
     int i = p >> lc, j = p & (core - 1);
     int sum = 0;
     for (int k = 0; k < qsize; k++) sum += (int)M[(k << lc) + j] * (int)sc.tmp[k * 33 + i];
-    int v = iclip((sum + add2) >> shift2, -32768, 32767);
+    int v = R.stage2(sum);
     if (rep == 1) block[i * bpitch + j] = (int16_t)v;
     else
       for (int m = 0; m < rep; m++)
@@ -1435,47 +1504,25 @@ __device__ void warp_inv_transform(const int16_t *coef, int cpitch, int size, in
 // two-state machine along the zig-zag scan; each lane simulates its 8-position chunk for both start states, a warp
 // scan composes the state maps, then each lane replays its chunk from the true start state.
 // ---------------------------------------------------------------------------------------------------------------
-__constant__ uint16_t c_quant[6] = {26214, 23302, 20560, 18396, 16384, 14564};  // common/common_tables.c:72
-__constant__ uint16_t c_dequant[6] = {40, 45, 51, 57, 64, 72};                  // common/common_tables.c:73
-
-// scan index of raster position (r,c) in an n x n zig-zag (common/common_tables.c:29-62), closed form
-__device__ __forceinline__ int zigzag_index(int r, int c, int n) {
-  int d = r + c;
-  int before = d < n ? d * (d + 1) / 2 : n * n - (2 * n - 1 - d) * (2 * n - d) / 2;  // samples on earlier diagonals
-  int lo = d < n ? 0 : d - (n - 1);  // smallest row index on this diagonal
-  // odd diagonals run top-right -> bottom-left (row ascending), even ones the other way
-  int k = (d & 1) ? (r - lo) : ((d < n ? d : n - 1) - r);
-  return before + k;
-}
-
-// T = int when every intermediate fits 32 bits (scale <= 26214, |coef| <= 32768 -> product < 2^30; offsets <= 115 << (shift2 - 8)
-// stay below 2^27 for shift2 <= 28), int64_t otherwise: same values, a third of the multiply instructions.
-template <class T> __device__ __forceinline__ int warp_quantize_t(const int16_t *coef, int16_t *coefq, int qp, int size, int coeff_type, TxScratch &sc, int shift2, const uint8_t *zz16) {
+__device__ int warp_quantize(const int16_t *coef, int16_t *coefq, int qp, int size, int coeff_type, TxScratch &sc, const uint8_t *zz16 = nullptr) {
   const int lane = lane_id();
-  const int intra = (coeff_type >> 1) & 1, qsize = min(size, 16), nq = qsize * qsize, lq = ilog2(qsize);
-  const T scale = c_quant[qp % 6];
+  const int qsize = min(size, 16), nq = qsize * qsize, lq = ilog2(qsize);
+  const Quantizer Q(qp, ilog2(size), coeff_type);
   int *scan = (int *)sc.in;  // reuse: 256 ints of scan-ordered coefficients
   const bool tab = zz16 != nullptr && qsize == 16;  // 16x16 scan positions from a shared-memory table instead of the closed form
   for (int p = lane; p < nq; p += 32) scan[tab ? (int)zz16[p] : zigzag_index(p >> lq, p & (qsize - 1), qsize)] = coef[p];
   __syncwarp();
-  // each lane owns `per` (<= 8) consecutive scan positions; their three candidate levels are computed ONCE and kept in registers:
-  // level0 = ac >> shift2 decides between the two rounding offsets, lvA / lvB are the levels with off0 / off1
-  const T unit = (T)1 << (shift2 - 8);
-  const T off_last = (T)(intra ? 38 : -26) * unit;
-  const T off0 = (T)(intra ? 102 : 51) * unit, off1 = (T)(intra ? 115 : 90) * unit;
+  // each lane owns `per` (<= 8) consecutive scan positions; their levels in both level modes are computed ONCE and kept in registers
   const int per = (nq + 31) / 32, p0 = lane * per;
-  int cv[8], l0[8], lvA[8], lvB[8];
+  int cv[8], lv0[8], lv1[8];
   int last = -1;
 #pragma unroll
   for (int t = 0; t < 8; t++) {
     const int p = p0 + t;
     cv[t] = (t < per && p < nq) ? scan[p] : 0;
-    const T ac = scale * (T)iabs(cv[t]);
-    l0[t] = (int)(ac >> shift2);
-    lvA[t] = (int)((ac + off0) >> shift2);
-    lvB[t] = (int)((ac + off1) >> shift2);
-    const T l = ac + off_last;
-    if (t < per && p < nq && (int)((l > 0 ? l : -l) >> shift2)) last = p;  // last_pos: highest position whose level with the "last" offset is non-zero
+    lv0[t] = Q.level(cv[t], 0);
+    lv1[t] = Q.level(cv[t], 1);
+    if (t < per && p < nq && Q.last_nz(cv[t])) last = p;
   }
   last = (int)__reduce_max_sync(FULL, (unsigned)(last + 1)) - 1;
   unsigned map = 0;  // bit s = end state when the chunk is entered in state s
@@ -1483,13 +1530,8 @@ template <class T> __device__ __forceinline__ int warp_quantize_t(const int16_t 
   for (int st = 0; st < 2; st++) {
     int mode = st;
 #pragma unroll
-    for (int t = 0; t < 8; t++) {
-      if (t < per && p0 + t <= last) {
-        const int level = (l0[t] > (1 - mode)) ? lvB[t] : lvA[t];
-        if (mode) { if (level == 0) mode = 0; }
-        else if (level > 1) mode = 1;
-      }
-    }
+    for (int t = 0; t < 8; t++)
+      if (t < per && p0 + t <= last) mode = Quantizer::next_mode(mode, mode ? lv1[t] : lv0[t]);
     map |= (unsigned)mode << st;
   }
   // inclusive scan of map composition: state after chunk L given state before chunk 0
@@ -1511,11 +1553,10 @@ template <class T> __device__ __forceinline__ int warp_quantize_t(const int16_t 
     if (t < per && p < nq) {
       int q = 0;
       if (p <= last) {
-        const int level = (l0[t] > (1 - mode)) ? lvB[t] : lvA[t];
+        const int level = mode ? lv1[t] : lv0[t];
         q = cv[t] < 0 ? -level : level;
         cbp |= level != 0;
-        if (mode) { if (level == 0) mode = 0; }
-        else if (level > 1) mode = 1;
+        mode = Quantizer::next_mode(mode, level);
       }
       sc.tmp[p] = (int16_t)q;  // scan order
     }
@@ -1524,10 +1565,6 @@ template <class T> __device__ __forceinline__ int warp_quantize_t(const int16_t 
   for (int p = lane; p < nq; p += 32) coefq[p] = sc.tmp[tab ? (int)zz16[p] : zigzag_index(p >> lq, p & (qsize - 1), qsize)];
   __syncwarp();
   return __any_sync(FULL, cbp);
-}
-__device__ int warp_quantize(const int16_t *coef, int16_t *coefq, int qp, int size, int coeff_type, TxScratch &sc, const uint8_t *zz16 = nullptr) {
-  const int shift2 = 21 - ilog2(size) + qp / 6;
-  return shift2 <= 28 ? warp_quantize_t<int>(coef, coefq, qp, size, coeff_type, sc, shift2, zz16) : warp_quantize_t<int64_t>(coef, coefq, qp, size, coeff_type, sc, shift2, zz16);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1609,7 +1646,7 @@ __device__ int warp_coeff_bits(const int16_t *scan, int nq, int size, int type) 
     if (last == 0 && iabs(scan[0]) == 1) return 2;
     bits = lane == 0 ? 1 : 0;
   }
-  // state map of the chunk for both entry states, composed across lanes (see warp_quantize_t)
+  // state map of the chunk for both entry states, composed across lanes (see warp_quantize)
   unsigned map = 0;
   for (int st = 0; st < 2; st++) {
     int S = st;
@@ -1707,7 +1744,7 @@ template <class S> __device__ __forceinline__ void store_row4(S *p, const int (&
 template <class S>
 __device__ int thread_txfm4(const S *orig, int os, const S *pred, int ps, S *rec, int rs, int16_t *coeffq_out, int qp, int coeff_type, int bitdepth,
                             uint64_t &ssd_out, int want_bits, int &bits_out) {
-  constexpr int ZZ[16] = {0, 1, 5, 6, 2, 4, 7, 12, 3, 8, 11, 13, 9, 10, 14, 15};  // raster -> scan (common/common_tables.c:29-34)
+  constexpr ZigZag<4> ZZ;
   const int maxv = (1 << bitdepth) - 1;
   int o[16], p[16], t[16], c[16];
 #pragma unroll
@@ -1718,72 +1755,59 @@ __device__ int thread_txfm4(const S *orig, int os, const S *pred, int ps, S *rec
 #pragma unroll
     for (int k = 0; k < 4; k++) { o[r * 4 + k] = a[k]; p[r * 4 + k] = b[k]; }
   }
-  // forward, 1st dimension: t[i][j] = (sum_k M[i][k] * res[j][k] + add1) >> shift1 (int16)
-  const int shift1 = bitdepth - 6, add1 = 1 << (shift1 - 1);
+  // forward, 1st dimension: t[i][j] = stage1(sum_k M[i][k] * res[j][k])
+  const FwdRound R(2, 0, bitdepth);
 #pragma unroll
   for (int j = 0; j < 4; j++) {
     int y0, y1, y2, y3;
     dct4_fwd(o[j * 4] - p[j * 4], o[j * 4 + 1] - p[j * 4 + 1], o[j * 4 + 2] - p[j * 4 + 2], o[j * 4 + 3] - p[j * 4 + 3], y0, y1, y2, y3);
-    t[0 * 4 + j] = (int16_t)((y0 + add1) >> shift1); t[1 * 4 + j] = (int16_t)((y1 + add1) >> shift1);
-    t[2 * 4 + j] = (int16_t)((y2 + add1) >> shift1); t[3 * 4 + j] = (int16_t)((y3 + add1) >> shift1);
+    t[0 * 4 + j] = R.stage1(y0); t[1 * 4 + j] = R.stage1(y1); t[2 * 4 + j] = R.stage1(y2); t[3 * 4 + j] = R.stage1(y3);
   }
-  // 2nd dimension: coef[i][j] = (sum_k M[i][k] * t[j][k] + 64) >> 7, stored straight into scan order
+  // 2nd dimension: coef[i][j] = stage2(sum_k M[i][k] * t[j][k]), stored straight into scan order
   int sc[16];
 #pragma unroll
   for (int j = 0; j < 4; j++) {
     int y0, y1, y2, y3;
     dct4_fwd(t[j * 4], t[j * 4 + 1], t[j * 4 + 2], t[j * 4 + 3], y0, y1, y2, y3);
-    sc[ZZ[0 * 4 + j]] = (int16_t)((y0 + 64) >> 7); sc[ZZ[1 * 4 + j]] = (int16_t)((y1 + 64) >> 7);
-    sc[ZZ[2 * 4 + j]] = (int16_t)((y2 + 64) >> 7); sc[ZZ[3 * 4 + j]] = (int16_t)((y3 + 64) >> 7);
+    sc[ZZ.pos[0 * 4 + j]] = R.stage2(y0); sc[ZZ.pos[1 * 4 + j]] = R.stage2(y1);
+    sc[ZZ.pos[2 * 4 + j]] = R.stage2(y2); sc[ZZ.pos[3 * 4 + j]] = R.stage2(y3);
   }
-  // quantize (enc/encode_block.c:84-160), size 4: shift2 = 19 + qp/6; products fit 32 bits (|c| * 26214 + offset < 2^31)
-  const int intra = (coeff_type >> 1) & 1, scale = c_quant[qp % 6], shift2 = 19 + qp / 6;
-  const int off_last = (intra ? 38 : -26) * (1 << (shift2 - 8));
+  const Quantizer Q(qp, 2, coeff_type);
   int last = -1;
 #pragma unroll
-  for (int pos = 0; pos < 16; pos++) {
-    int l = iabs(sc[pos]) * scale + off_last;
-    if ((iabs(l) >> shift2) != 0) last = pos;
-  }
-  const int off0 = (intra ? 102 : 51) << (shift2 - 8), off1 = (intra ? 115 : 90) << (shift2 - 8);
+  for (int pos = 0; pos < 16; pos++)
+    if (Q.last_nz(sc[pos])) last = pos;
   int mode = 1, cbp = 0, q[16];
 #pragma unroll
   for (int pos = 0; pos < 16; pos++) {
     int lev = 0;
     if (pos <= last) {
-      int ac = scale * iabs(sc[pos]);
-      int level0 = ac >> shift2;
-      lev = (ac + ((level0 > (1 - mode)) ? off1 : off0)) >> shift2;
+      lev = Q.level(sc[pos], mode);
       cbp |= lev != 0;
-      if (mode) { if (lev == 0) mode = 0; }
-      else if (lev > 1) mode = 1;
+      mode = Quantizer::next_mode(mode, lev);
     }
     q[pos] = sc[pos] < 0 ? -lev : lev;
   }
   if (coeffq_out) {
 #pragma unroll
-    for (int r = 0; r < 16; r++) coeffq_out[r] = (int16_t)q[ZZ[r]];
+    for (int r = 0; r < 16; r++) coeffq_out[r] = (int16_t)q[ZZ.pos[r]];
   }
   bits_out = (want_bits && cbp) ? thread_coeff_bits<16>(q, 4, coeff_type) : 0;
   uint64_t ssd = 0;
   if (cbp) {
-    // dequantize (common/common_block.c:45-73), size 4: rshift = 1
-    const int lshift = qp / 6, dscale = c_dequant[qp % 6];
+    const Dequantizer D(qp, 2);
 #pragma unroll
-    for (int r = 0; r < 16; r++) {
-      int v = q[ZZ[r]] * dscale;
-      c[r] = lshift >= 1 ? (int)(int16_t)((unsigned)v << (lshift - 1)) : (int)(int16_t)((v + 1) >> 1);
-    }
-    // inverse, 1st dimension: t[i][j] = clip16((sum_k M[k][j] * c[k][i] + 64) >> 7)
+    for (int r = 0; r < 16; r++) c[r] = D(q[ZZ.pos[r]]);
+    // inverse, 1st dimension: t[i][j] = stage1(sum_k M[k][j] * c[k][i])
 #pragma unroll
     for (int i = 0; i < 4; i++) {
       int y0, y1, y2, y3;
       dct4_inv(c[0 * 4 + i], c[1 * 4 + i], c[2 * 4 + i], c[3 * 4 + i], y0, y1, y2, y3);
-      t[i * 4 + 0] = iclip((y0 + 64) >> 7, -32768, 32767); t[i * 4 + 1] = iclip((y1 + 64) >> 7, -32768, 32767);
-      t[i * 4 + 2] = iclip((y2 + 64) >> 7, -32768, 32767); t[i * 4 + 3] = iclip((y3 + 64) >> 7, -32768, 32767);
+      t[i * 4 + 0] = InvRound::stage1(y0); t[i * 4 + 1] = InvRound::stage1(y1);
+      t[i * 4 + 2] = InvRound::stage1(y2); t[i * 4 + 3] = InvRound::stage1(y3);
     }
-    // 2nd dimension + reconstruction: out[i][j] = clip16((sum_k M[k][j] * t[k][i] + add2) >> (20 - bitdepth))
-    const int shiftB = 20 - bitdepth, addB = 1 << (shiftB - 1);
+    // 2nd dimension + reconstruction: out[i][j] = stage2(sum_k M[k][j] * t[k][i])
+    const InvRound RI(bitdepth);
 #pragma unroll
     for (int i = 0; i < 4; i++) {
       int y[4];
@@ -1791,7 +1815,7 @@ __device__ int thread_txfm4(const S *orig, int os, const S *pred, int ps, S *rec
       int v[4];
 #pragma unroll
       for (int j = 0; j < 4; j++) {
-        int r = iclip((y[j] + addB) >> shiftB, -32768, 32767);
+        int r = RI.stage2(y[j]);
         v[j] = sat_px(r + p[i * 4 + j], maxv);
         int d = o[i * 4 + j] - v[j];
         ssd += (uint32_t)(d * d);
@@ -1819,8 +1843,7 @@ __device__ int thread_txfm4(const S *orig, int os, const S *pred, int ps, S *rec
 // interleaves per thread, so the lock-step (uniform-index) accesses of a warp coalesce into L1 lines; the DCT matrix is
 // read from the shared-memory table with a warp-uniform index (broadcast).  Same arithmetic as warp_fwd_transform /
 // warp_quantize / warp_dequantize / warp_inv_transform.
-__constant__ uint8_t c_zz8[64] = {0,  1,  5,  6,  14, 15, 27, 28, 2,  4,  7,  13, 16, 26, 29, 42, 3,  8,  12, 17, 25, 30, 41, 43, 9,  11, 18, 24, 31, 40, 44, 53,
-                                   10, 19, 23, 32, 39, 45, 52, 54, 20, 22, 33, 38, 46, 51, 55, 60, 21, 34, 37, 47, 50, 56, 59, 61, 35, 36, 48, 49, 57, 58, 62, 63};
+__constant__ ZigZag<8> c_zz8;  // not const: a const table is folded into the code, which costs thread_txfm8 spills
 // eight-term dot product of an int8 matrix row (two words) with eight int16 values (four words): four DP2A
 __device__ __forceinline__ int dot8(uint2 m, uint4 v, int acc) {
   acc = __dp2a_lo((int)v.x, (int)m.x, acc);
@@ -1841,60 +1864,50 @@ __device__ int thread_txfm8(const S *orig, int os, const S *pred, int ps, S *rec
     *(uint4 *)&a[r * 8] = make_uint4(((uint32_t)(o0[0] - p0[0]) & 0xffffu) | ((uint32_t)(o0[1] - p0[1]) << 16), ((uint32_t)(o0[2] - p0[2]) & 0xffffu) | ((uint32_t)(o0[3] - p0[3]) << 16),
                                      ((uint32_t)(o1[0] - p1[0]) & 0xffffu) | ((uint32_t)(o1[1] - p1[1]) << 16), ((uint32_t)(o1[2] - p1[2]) & 0xffffu) | ((uint32_t)(o1[3] - p1[3]) << 16));
   }
-  // forward: b[i][j] = (M[i] . res[j] + add1) >> shift1, then a[scan(i, j)] = (M[i] . b[j] + 128) >> 8
-  const int shift1 = 3 + bitdepth - 8, add1 = 1 << (shift1 - 1);
+  // forward: b[i][j] = stage1(M[i] . res[j]), then a[scan(i, j)] = stage2(M[i] . b[j])
+  const FwdRound R(3, 0, bitdepth);
   for (int j = 0; j < 8; j++) {
     const uint4 v = *(const uint4 *)&a[j * 8];
 #pragma unroll
-    for (int i = 0; i < 8; i++) b[i * 8 + j] = (int16_t)(dot8(M[i], v, add1) >> shift1);
+    for (int i = 0; i < 8; i++) b[i * 8 + j] = (int16_t)R.stage1(dot8(M[i], v, 0));
   }
   for (int j = 0; j < 8; j++) {
     const uint4 v = *(const uint4 *)&b[j * 8];
 #pragma unroll
-    for (int i = 0; i < 8; i++) a[c_zz8[i * 8 + j]] = (int16_t)(dot8(M[i], v, 128) >> 8);  // scan order
+    for (int i = 0; i < 8; i++) a[c_zz8.pos[i * 8 + j]] = (int16_t)R.stage2(dot8(M[i], v, 0));  // scan order
   }
-  const int intra = (coeff_type >> 1) & 1, scale = c_quant[qp % 6], shift2 = 18 + qp / 6;
-  const int off_last = (intra ? 38 : -26) * (1 << (shift2 - 8));
+  const Quantizer Q(qp, 3, coeff_type);
   int last = -1;
-  for (int pos = 0; pos < 64; pos++) {
-    int l = iabs((int)a[pos]) * scale + off_last;
-    if ((iabs(l) >> shift2) != 0) last = pos;
-  }
-  const int off0 = (intra ? 102 : 51) << (shift2 - 8), off1 = (intra ? 115 : 90) << (shift2 - 8);
+  for (int pos = 0; pos < 64; pos++)
+    if (Q.last_nz(a[pos])) last = pos;
   int mode = 1, cbp = 0;
   for (int pos = 0; pos < 64; pos++) {
     int lev = 0, cc = a[pos];
     if (pos <= last) {
-      int ac = scale * iabs(cc);
-      int level0 = ac >> shift2;
-      lev = (ac + ((level0 > (1 - mode)) ? off1 : off0)) >> shift2;
+      lev = Q.level(cc, mode);
       cbp |= lev != 0;
-      if (mode) { if (lev == 0) mode = 0; }
-      else if (lev > 1) mode = 1;
+      mode = Quantizer::next_mode(mode, lev);
     }
     b[pos] = (int16_t)(cc < 0 ? -lev : lev);  // quantised, scan order
   }
   if (coeffq_out)
-    for (int p = 0; p < 64; p++) coeffq_out[p] = b[c_zz8[p]];
+    for (int p = 0; p < 64; p++) coeffq_out[p] = b[c_zz8.pos[p]];
   bits_out = (want_bits && cbp) ? thread_coeff_bits<64>(b, 8, coeff_type) : 0;
   uint64_t ssd = 0;
   if (cbp) {
     // de-quantise into the TRANSPOSED block a[i][k] = rcoeff[k][i], so that both inverse stages are row . row products
-    const int lshift = qp / 6, dscale = c_dequant[qp % 6];  // rshift = 2
+    const Dequantizer D(qp, 3);
     for (int k = 0; k < 8; k++)
 #pragma unroll
-      for (int i = 0; i < 8; i++) {
-        int v = (int)b[c_zz8[k * 8 + i]] * dscale;
-        a[i * 8 + k] = lshift >= 2 ? (int16_t)((unsigned)v << (lshift - 2)) : (int16_t)((v + (1 << (1 - lshift))) >> (2 - lshift));
-      }
-    // inverse 1st dimension: T[i][j] = clip16((sum_k M[k][j] * rcoeff[k][i] + 64) >> 7), stored transposed: b[j][i]
+      for (int i = 0; i < 8; i++) a[i * 8 + k] = (int16_t)D(b[c_zz8.pos[k * 8 + i]]);
+    // inverse 1st dimension: T[i][j] = stage1(sum_k M[k][j] * rcoeff[k][i]), stored transposed: b[j][i]
     for (int i = 0; i < 8; i++) {
       const uint4 v = *(const uint4 *)&a[i * 8];
 #pragma unroll
-      for (int j = 0; j < 8; j++) b[j * 8 + i] = (int16_t)iclip(dot8(Mt[j], v, 64) >> 7, -32768, 32767);
+      for (int j = 0; j < 8; j++) b[j * 8 + i] = (int16_t)InvRound::stage1(dot8(Mt[j], v, 0));
     }
-    // 2nd dimension + reconstruction: out[i][j] = clip16((sum_k M[k][j] * T[k][i] + addB) >> shiftB) = Mt[j] . b[i]
-    const int shiftB = 20 - bitdepth, addB = 1 << (shiftB - 1);
+    // 2nd dimension + reconstruction: out[i][j] = stage2(sum_k M[k][j] * T[k][i]) = stage2(Mt[j] . b[i])
+    const InvRound RI(bitdepth);
     for (int i = 0; i < 8; i++) {
       const uint4 v = *(const uint4 *)&b[i * 8];
 #pragma unroll
@@ -1904,7 +1917,7 @@ __device__ int thread_txfm8(const S *orig, int os, const S *pred, int ps, S *rec
         load_row4<S>(orig + i * os + 4 * h2, ov);
 #pragma unroll
         for (int t = 0; t < 4; t++) {
-          int r = iclip(dot8(Mt[4 * h2 + t], v, addB) >> shiftB, -32768, 32767);
+          int r = RI.stage2(dot8(Mt[4 * h2 + t], v, 0));
           o4[t] = sat_px(r + pv[t], maxv);
           int d = ov[t] - o4[t];
           ssd += (uint32_t)(d * d);
@@ -1930,13 +1943,9 @@ __device__ int thread_txfm8(const S *orig, int os, const S *pred, int ps, S *rec
 
 // a13: dequantize.  common/common_block.c:45-73 (no weight matrix).  compact in, compact out (pitch qsize)
 __device__ void warp_dequantize(const int16_t *cq, int16_t *rc, int qp, int size) {
-  const int lshift = qp / 6, qsize = min(size, 16), rshift = ilog2(size) - 1;
-  const int64_t scale = c_dequant[qp % 6];
-  const int64_t add = lshift < rshift ? (1 << (rshift - lshift - 1)) : 0;
-  for (int p = lane_id(); p < qsize * qsize; p += 32) {
-    int c = cq[p];
-    rc[p] = lshift >= rshift ? (int16_t)((c * scale) << (lshift - rshift)) : (int16_t)((c * scale + add) >> (rshift - lshift));
-  }
+  const int qsize = min(size, 16);
+  const Dequantizer D(qp, ilog2(size));
+  for (int p = lane_id(); p < qsize * qsize; p += 32) rc[p] = (int16_t)D(cq[p]);
   __syncwarp();
 }
 

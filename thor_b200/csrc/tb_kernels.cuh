@@ -373,9 +373,8 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
   const bool dct_warp = TW == 1 || threadIdx.x < 32;
   const int ia = lane >> 3, jb = lane & 7;
   {
-    const int shift1 = ilog2(size) + ilog2(scale) + bitdepth - 8, add1 = 1 << (shift1 - 1);
-    const int shift2 = l1 + 5, add2 = 1 << (shift2 - 1);
-    // tmp[i][j] = (M[i][.] . in[j][.] + add1) >> shift1   (i < 16, j < size1)
+    const FwdRound R(ilog2(size), ilog2(scale), bitdepth);
+    // tmp[i][j] = stage1(M[i][.] . in[j][.])   (i < 16, j < size1)
     if (dct_warp) {
       if (size1 == 16) {
         int acc[4][2] = {};
@@ -383,7 +382,7 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
 #pragma unroll
         for (int r = 0; r < 4; r++)
 #pragma unroll
-          for (int c = 0; c < 2; c++) sc.tmp[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)((acc[r][c] + add1) >> shift1);
+          for (int c = 0; c < 2; c++) sc.tmp[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)R.stage1(acc[r][c]);
       } else {
         int acc[4][4] = {};
         dot16_block<4, 4>(M1 + 4 * ia * mp1, mp1, sc.in + jb * PI, 8 * PI, acc);
@@ -391,11 +390,11 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
 #pragma unroll
         for (int r = 0; r < 4; r++)
 #pragma unroll
-          for (int c = 0; c < 4; c++) sc.tmp[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)((acc[r][c] + add1) >> shift1);
+          for (int c = 0; c < 4; c++) sc.tmp[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)R.stage1(acc[r][c]);
       }
     }
     sync();
-    // coef[i][j] = (M[i][.] . tmp[j][.] + add2) >> shift2  (i, j < 16)
+    // coef[i][j] = stage2(M[i][.] . tmp[j][.])  (i, j < 16)
     if (dct_warp) {
       int acc[4][2] = {};
       dot16_block<4, 2>(M1 + 4 * ia * mp1, mp1, sc.tmp + jb * PI, 8 * PI, acc);
@@ -403,7 +402,7 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
 #pragma unroll
       for (int r = 0; r < 4; r++)
 #pragma unroll
-        for (int c = 0; c < 2; c++) sc.rc[(4 * ia + r) * 16 + jb + 8 * c] = (int16_t)((acc[r][c] + add2) >> shift2);
+        for (int c = 0; c < 2; c++) sc.rc[(4 * ia + r) * 16 + jb + 8 * c] = (int16_t)R.stage2(acc[r][c]);
     }
     sync();
   }
@@ -426,21 +425,19 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
     // de-quantise (common/common_block.c:45-73) straight into the TRANSPOSED tile in[i][k] = rcoeff[k][i], so that the
     // inverse transform's sums over k read contiguous int16 pairs
     {
-      const int lshift = q.qp / 6, rshift = ilog2(size) - 1;
-      const int dscale = c_dequant[q.qp % 6];  // |c * dscale| <= 32768 * 72 and the shift is <= qp / 6: 32-bit arithmetic is exact
-      const int dadd = lshift < rshift ? (1 << (rshift - lshift - 1)) : 0;
+      const Dequantizer D(q.qp, ilog2(size));
       for (int p = tid; p < qsize * qsize; p += NT) {
-        int k = p >> lq, i = p & (qsize - 1), c = sc.cq[p];
-        sc.in[i * PI + k] = lshift >= rshift ? (int16_t)((unsigned)(c * dscale) << (lshift - rshift)) : (int16_t)((c * dscale + dadd) >> (rshift - lshift));
+        int k = p >> lq, i = p & (qsize - 1);
+        sc.in[i * PI + k] = (int16_t)D(sc.cq[p]);
       }
       sync();
     }
     // inverse transform with the reconstruction (common/common_block.c:75-83) and SSD fused into its output stage
     const int core = min(size, 32), rep = size / core, lc = ilog2(core);
-    const int shiftB = 20 - bitdepth, addB = 1 << (shiftB - 1);
+    const InvRound RI(bitdepth);
     const int8_t *Mt = tab8t + dct_tab8_ofs(lc);
     const int mpc = dct_tab8_pitch(lc);
-    // T[i][j] = clip16((sum_k M[k][j] * rcoeff[k][i] + 64) >> 7), stored transposed: tmp2[j][i]   (i < 16, j < core)
+    // T[i][j] = stage1(sum_k M[k][j] * rcoeff[k][i]), stored transposed: tmp2[j][i]   (i < 16, j < core)
     int16_t *tmp2 = sc.in + 16 * PI;  // rows 16.. of the `in` tile are free here (rcoeff^T uses rows 0..15)
     if (dct_warp) {
       if (core == 16) {
@@ -449,7 +446,7 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
 #pragma unroll
         for (int r = 0; r < 4; r++)
 #pragma unroll
-          for (int c = 0; c < 2; c++) tmp2[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)iclip((acc[r][c] + 64) >> 7, -32768, 32767);
+          for (int c = 0; c < 2; c++) tmp2[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)InvRound::stage1(acc[r][c]);
       } else {
 #pragma unroll
         for (int half = 0; half < 2; half++) {
@@ -458,12 +455,12 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
 #pragma unroll
           for (int r = 0; r < 4; r++)
 #pragma unroll
-            for (int c = 0; c < 2; c++) tmp2[(16 * half + 4 * ia + r) * PI + jb + 8 * c] = (int16_t)iclip((acc[r][c] + 64) >> 7, -32768, 32767);
+            for (int c = 0; c < 2; c++) tmp2[(16 * half + 4 * ia + r) * PI + jb + 8 * c] = (int16_t)InvRound::stage1(acc[r][c]);
         }
       }
     }
     sync();
-    // out[i][j] = clip16((sum_k M[k][j] * T[k][i] + addB) >> shiftB) = Mt[j][.] . tmp2[i][.]   (i, j < core); lane (jg = lane >> 3,
+    // out[i][j] = stage2(sum_k M[k][j] * T[k][i]) = stage2(Mt[j][.] . tmp2[i][.])   (i, j < core); lane (jg = lane >> 3,
     // il = lane & 7) owns columns 4 jg .. 4 jg + 3 (+16 in a second pass for core 32) of rows il, il + 8, ..
     if (rep == 1) {
       if (dct_warp) {
@@ -479,7 +476,7 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
               load_row4<S>(orig + i * q.ostride + j, ov);
 #pragma unroll
               for (int t = 0; t < 4; t++) {
-                int r = iclip((acc[t][c] + addB) >> shiftB, -32768, 32767);
+                int r = RI.stage2(acc[t][c]);
                 v[t] = sat_px(r + pv[t], maxv);
                 int d = ov[t] - v[t];
                 ssd += (uint64_t)(uint32_t)(d * d);
@@ -499,7 +496,7 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
 #pragma unroll
             for (int c = 0; c < 2; c++)
 #pragma unroll
-              for (int t = 0; t < 4; t++) rt[(i0 + 8 * c) * PI + 4 * jg + t] = (int16_t)iclip((acc[t][c] + addB) >> shiftB, -32768, 32767);
+              for (int t = 0; t < 4; t++) rt[(i0 + 8 * c) * PI + 4 * jg + t] = (int16_t)RI.stage2(acc[t][c]);
           }
         }
       }
@@ -523,7 +520,7 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
       for (int p = tid; p < core * core; p += NT) {
         int i = p >> lc, j = p & (core - 1);
         int sum = dot_s8_s16(Mt + j * mpc, tmp2 + i * PI, qsize);
-        int r = iclip((sum + addB) >> shiftB, -32768, 32767);
+        int r = RI.stage2(sum);
         for (int m = 0; m < rep; m++)
           for (int nn = 0; nn < rep; nn++) {
             int y = i * rep + m, x = j * rep + nn;

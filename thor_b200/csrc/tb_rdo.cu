@@ -315,7 +315,7 @@ template <class S> struct DevBackend {
       if (e < N * N) { const int i = e >> ln, j = e & (N - 1); A[w] = (int16_t)((int)q.orig[i * q.os + j] - (int)q.pred[i * q.ps + j]); }
     }
     sync();
-    // (2) forward, first dimension: B[k][i][j] = (sum_t M[i][t] * A[k][j][t] + add1) >> shift1
+    // (2) forward, first dimension: B[k][i][j] = stage1(sum_t M[i][t] * A[k][j][t])
     TB_ROLL
     for (int w = l; w < n * 64; w += 32) {
       const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
@@ -325,12 +325,11 @@ template <class S> struct DevBackend {
         int sum = 0;
         TB_ROLL
         for (int t = 0; t < N; t++) sum += (int)M[t] * (int)a[t];
-        const int shift1 = ln + bd - 8;
-        B[w] = (int16_t)((sum + (1 << (shift1 - 1))) >> shift1);
+        B[w] = (int16_t)FwdRound(ln, 0, bd).stage1(sum);
       }
     }
     sync();
-    // (3) forward, second dimension: A[k][i][j] = (sum_t M[i][t] * B[k][j][t] + add2) >> shift2   (coefficients, raster)
+    // (3) forward, second dimension: A[k][i][j] = stage2(sum_t M[i][t] * B[k][j][t])   (coefficients, raster)
     TB_ROLL
     for (int w = l; w < n * 64; w += 32) {
       const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
@@ -341,8 +340,7 @@ template <class S> struct DevBackend {
         int sum = 0;
         TB_ROLL
         for (int t = 0; t < N; t++) sum += (int)M[t] * (int)b[t];
-        const int shift2 = ln + 5;
-        v = (sum + (1 << (shift2 - 1))) >> shift2;
+        v = FwdRound(ln, 0, bd).stage2(sum);
       }
       if (e < N * N) A[w] = (int16_t)v;  // A was consumed by (2)
     }
@@ -358,28 +356,20 @@ template <class S> struct DevBackend {
     int cbp = 0;
     if (l < n) {
       const tbr::TxJob<S> &q = J[l];
-      const int N = q.size, nq = N * N, intra = (q.coeff_type >> 1) & 1, scale = c_quant[q.qp % 6], shift2 = 21 - (N == 8 ? 3 : 2) + q.qp / 6;
+      const int N = q.size, nq = N * N;
+      const Quantizer Q(q.qp, N == 8 ? 3 : 2, q.coeff_type);
       int16_t *sc_ = B + (l << 6);
-      const int offset = (intra ? 38 : -26) * (1 << (shift2 - 8));
-      int level = 0, pos = nq - 1;
-      while (level == 0 && pos >= 0) {
-        const int v = iabs((int)sc_[pos]) * scale + offset;  // < 2^31: |c| <= 32768, scale <= 26214
-        level = iabs(v) >> shift2;
-        pos--;
-      }
-      const int last_pos = level ? pos + 1 : pos;
-      const int off0 = (intra ? 102 : 51) << (shift2 - 8), off1 = (intra ? 115 : 90) << (shift2 - 8);
+      bool nz = false;
+      int pos = nq - 1;
+      while (!nz && pos >= 0) nz = Q.last_nz(sc_[pos--]);
+      const int last_pos = nz ? pos + 1 : pos;
       int level_mode = 1;
       TB_ROLL
       for (pos = 0; pos <= last_pos; pos++) {
-        const int c = sc_[pos];
-        const unsigned ac = (unsigned)scale * (unsigned)iabs(c);
-        const int level0 = (int)(ac >> shift2);
-        const int lev = (int)((ac + (unsigned)((level0 > (1 - level_mode)) ? off1 : off0)) >> shift2);
+        const int c = sc_[pos], lev = Q.level(c, level_mode);
         sc_[pos] = (int16_t)(c < 0 ? -lev : lev);
         cbp |= lev != 0;
-        if (level_mode) { if (lev == 0) level_mode = 0; }
-        else if (lev > 1) level_mode = 1;
+        level_mode = Quantizer::next_mode(level_mode, lev);
       }
       TB_ROLL
       for (pos = last_pos + 1; pos < nq; pos++) sc_[pos] = 0;
@@ -395,12 +385,11 @@ template <class S> struct DevBackend {
       if (e < N * N) {
         const int c = B[(k << 6) + zigzag_index(e >> ln, e & (N - 1), N)];
         q.cq[e] = (int16_t)c;
-        const int lshift = q.qp / 6, rshift = ln - 1, dscale = c_dequant[q.qp % 6];
-        A[w] = lshift >= rshift ? (int16_t)((c * dscale) << (lshift - rshift)) : (int16_t)((c * dscale + (1 << (rshift - lshift - 1))) >> (rshift - lshift));
+        A[w] = (int16_t)Dequantizer(q.qp, ln)(c);
       }
     }
     sync();
-    // (7) inverse, first dimension: B[k][i][j] = sat16((sum_t M[t][j] * A[k][t][i] + 64) >> 7)
+    // (7) inverse, first dimension: B[k][i][j] = stage1(sum_t M[t][j] * A[k][t][i])
     TB_ROLL
     for (int w = l; w < n * 64; w += 32) {
       const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
@@ -410,12 +399,11 @@ template <class S> struct DevBackend {
         int o = 0;
         TB_ROLL
         for (int t = 0; t < N; t++) o += (int)M[(t << ln) + j] * (int)a[(t << ln) + i];
-        o = (o + 64) >> 7;
-        B[w] = (int16_t)iclip(o, -32768, 32767);
+        B[w] = (int16_t)InvRound::stage1(o);
       }
     }
     sync();
-    // (8) inverse, second dimension + reconstruction: rec = clip(pred + sat16((sum_t M[t][j] * B[k][t][i] + round) >> (20 - bitdepth))); no coefficient: rec = pred
+    // (8) inverse, second dimension + reconstruction: rec = clip(pred + stage2(sum_t M[t][j] * B[k][t][i])); no coefficient: rec = pred
     TB_ROLL
     for (int w = l; w < n * 64; w += 32) {
       const int k = w >> 6, e = w & 63;
@@ -429,9 +417,7 @@ template <class S> struct DevBackend {
           int o = 0;
           TB_ROLL
           for (int t = 0; t < N; t++) o += (int)M[(t << ln) + j] * (int)b[(t << ln) + i];
-          const int sh2 = 20 - bd;
-          o = (o + (1 << (sh2 - 1))) >> sh2;
-          v = sat_px(v + iclip(o, -32768, 32767), maxv);
+          v = sat_px(v + InvRound(bd).stage2(o), maxv);
         }
         q.rec[i * q.rs + j] = (S)v;
       }
