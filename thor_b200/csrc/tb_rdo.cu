@@ -40,7 +40,7 @@ enum { PF_INTERP, PF_ME, PF_MEBI, PF_TX, PF_BITS, PF_SSD, PF_INTRA, PF_COPY, PF_
 enum { ST_ME = PF_N, ST_ME_INT, ST_ME_SUB, ST_ME_SAMPLES, ST_IP, ST_IP_SAMPLES, ST_TX, ST_TX_SAMPLES, ST_INTRA, ST_INTRA_SAMPLES, ST_SSD_SAMPLES, ST_SB,
        ST_ME_SZ /* cycles of searches by coding-block size 8..128 */, ST_TX_SZ = ST_ME_SZ + 5 /* chains by transform size 4..128 */, ST_IP_SZ = ST_TX_SZ + 6 /* predictions by width 4..128 */,
        ST_PH = ST_IP_SZ + 6 /* wall cycles of warp 0 by decision phase (tb_rdo.h PH_*) */, ST_MESTAGE = ST_PH + tbr::PH_N /* search stages, coding blocks <= 16 */,
-       ST_X = ST_MESTAGE + 5 /* search phase of a block decision: warp 0 {own searches, -, barrier wait}, warp nw-1 {-, intra items, barrier wait} */, ST_END = ST_X + 6 };
+       ST_X = ST_MESTAGE + 5 /* search phase of a block decision: warp 0 {own searches, -, barrier wait}, warp nw-1 {own searches, -, barrier wait} */, ST_END = ST_X + 6 };
 struct Prof {
   long long *acc;
   int k, k2;
@@ -974,8 +974,8 @@ int tb_rdo_batch_sync(tb_rdo_batch_t *b) {
       fprintf(stderr, "\n[tb_rdo prof] search stages (coding blocks <= 16):");
       for (int k = 0; k < 5; k++) fprintf(stderr, " %s %.1f%%", stg[k], 100.0 * (double)pr[ST_MESTAGE + k] / (double)(tot ? tot : 1));
     }
-    fprintf(stderr, "\n[tb_rdo prof] search phase: warp 0 own searches %.0f, (intra items %.0f), barrier wait %.0f | last warp (searches %.0f) intra items %.0f, barrier wait %.0f  [Mcycles]",
-            pr[ST_X] / 1e6, pr[ST_X + 1] / 1e6, pr[ST_X + 2] / 1e6, pr[ST_X + 3] / 1e6, pr[ST_X + 4] / 1e6, pr[ST_X + 5] / 1e6);
+    fprintf(stderr, "\n[tb_rdo prof] search phase: warp 0 own searches %.0f, barrier wait %.0f | last warp own searches %.0f, barrier wait %.0f  [Mcycles]",
+            pr[ST_X] / 1e6, pr[ST_X + 2] / 1e6, pr[ST_X + 3] / 1e6, pr[ST_X + 5] / 1e6);
     fprintf(stderr, "\n[tb_rdo prof] search cycles by coding-block size 8..128:");
     for (int k = 0; k < 5; k++) fprintf(stderr, " %.1f%%", 100.0 * (double)pr[ST_ME_SZ + k] / (double)(pr[PF_ME] ? pr[PF_ME] : 1));
     fprintf(stderr, "; transform chains by size 4..128:");

@@ -784,10 +784,14 @@ template <class S, class B> struct Rdo {
   // mode_decision_rdo :1835-2120.  The candidates in the reference's order: skip, merge x tb_param, inter (reference x partition x tb_param), bipred,
   // the joint bipred of B frames, intra x tb_param; the warps deal them round robin by their position in the group.
   // Square blocks of inter frames at encoder_speed 0 on more than one warp OVERLAP the sections that do not depend on each other instead:
-  //   while the references' motion searches run (one warp per reference), the remaining warps start the intra-mode search;
+  //   the references' motion searches run one warp per reference, and nothing else runs beside them;
   //   then warp 0 runs the bi-prediction chain (every search depends on the previous one) and evaluates its candidates, while the others draw the
-  //   inter candidates (one draw = the tb_param variants of one prediction) and the rest of the intra-mode search from shared counters;
-  //   the candidate lists the chain extends are copied to the other warps' replicas afterwards.
+  //   inter candidates (one draw = the tb_param variants of one prediction) from a shared counter;
+  //   after a barrier every warp draws the items of the intra-mode search, and the candidate lists the chain extends are copied to the other
+  //   warps' replicas.
+  // The RD loop is bound by instruction delivery: warps that run different code at the same time slow each other down (searches beside the
+  // intra-mode search take about 1.5 times the cycles of searches alone), while a warp waiting at a barrier fetches nothing.  So the intra-mode search,
+  // which no search and no inter candidate needs, runs neither beside the searches nor beside the chain, but in a section of its own.
   // The schedule decides only which warp evaluates what, and when: the winner = min (cost, index) is the reference's "first candidate with the
   // strictly smallest cost" either way.
   TBR_HD TBR_NI uint32_t mode_decision_rdo(BlockInfo &bi, int *owner) {
@@ -845,12 +849,7 @@ template <class S, class B> struct Rdo {
           sad_inter_r[ref_idx] = sad_inter;
           be.put_me(ref_idx, &mv_all[ref_idx][0][0], sad_inter);
         }
-        if (overlap) {  // the warps without a reference begin the intra-mode search
-          be.mark2(0);
-          if (be.warp() >= nrs)
-            for (int k; (k = be.next(1)) < n_isearch;) intra_search_item(bi, t, k, &my_icost, &my_ik);
-          be.mark2(1);
-        }
+        if (overlap) be.mark2(0);
         be.cta_sync();
         if (overlap) be.mark2(2);  // (diagnostics) the wait for the slowest warp of the phase
         // (2) every warp learns the other references' vectors and replays their effect on its replica of the candidate lists
@@ -880,7 +879,8 @@ template <class S, class B> struct Rdo {
           eval_tbs(bi, t, min_tb, IDX_INTER + g * ntb + min_tb + 1, overlap, &pos, true);
         }
         be.mark(PH_INTER_CAND);
-        if (overlap) {  // the rest of the intra-mode search
+        if (overlap) {  // the intra-mode search, once the chain and the inter candidates are done
+          be.cta_sync();
           for (int k; (k = be.next(1)) < n_isearch;) intra_search_item(bi, t, k, &my_icost, &my_ik);
           be.mark(PH_INTRA_SEARCH);
         }

@@ -7,6 +7,7 @@ import argparse
 import ctypes as C
 import json
 import os
+import re
 import sys
 import time
 
@@ -15,6 +16,13 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
+
+# the counters behind bench.py's (include/thor_b200.h TB_RDO_NSTATS): the search phase of an overlapped block decision (tb_rdo.cu ST_X), warp 0 and the last
+# warp, each {own searches, (unused), wait at the barrier that ends the phase}
+SEARCH_PHASE_NAMES = ["w0_own_searches", "w0_barrier_wait", "wlast_own_searches", "wlast_barrier_wait"]
+STAT_NAMES = bench.STAT_NAMES + ["x_w0_own_searches", "x_unused_1", "x_w0_barrier_wait", "x_wlast_own_searches", "x_unused_4", "x_wlast_barrier_wait"]
+NSTATS = int(re.search(r"#define TB_RDO_NSTATS (\d+)", open(os.path.join(ROOT, "include", "thor_b200.h")).read()).group(1))
+assert len(STAT_NAMES) == NSTATS, (len(STAT_NAMES), NSTATS)
 
 
 def main():
@@ -62,16 +70,17 @@ def main():
             assert L.tb_rdo_batch_download(b, s, C.byref(hf.desc)) == 0
         assert L.tb_rdo_batch_sync(b) == 0, L.tb_rdo_last_error()
         dt = time.time() - t
-    st = (C.c_uint64 * len(bench.STAT_NAMES))()
-    L.tb_rdo_batch_stats(b, st, len(st))
-    d = dict(zip(bench.STAT_NAMES, [int(v) for v in st]))
+    st = (C.c_uint64 * NSTATS)()
+    assert L.tb_rdo_batch_stats(b, st, NSTATS) == NSTATS
+    d = dict(zip(STAT_NAMES, [int(v) for v in st]))
     px = sum(hf.job.pixels for hf in hosts)
     ok = all(all(hf.check().values()) for hf in hosts)
     out = {"size": args.size, "frames": len(hosts), "ctas": int(L.tb_rdo_batch_grid(b)), "seconds": round(dt, 3), "mpixel_s": round(px / dt / 1e6, 4), "parity_ok": ok,
            "cycles_per_search": round(d["cyc_me"] / max(1, d["searches"])), "cycles_per_txfm_chain": round(d["cyc_tx_chain"] / max(1, d["txfm_chains"])),
            "cycles_per_prediction": round(d["cyc_interp"] / max(1, d["predictions"])), "cycles_per_intra": round(d["cyc_intra"] / max(1, d["intra_predictions"])),
            "warp_cycles_per_super_block": round(d["cyc_total"] * (1 - d["cyc_idle"] / max(1, d["cyc_total"])) / max(1, d["super_blocks"])),
-           "share": {k[4:]: round(d[k] / max(1, d["cyc_total"]), 4) for k in bench.STAT_NAMES[:10] + bench.STAT_NAMES[23:40]}, "phase": {k[3:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[40:49])), 4) for k in bench.STAT_NAMES[40:49]}, "me_stage": {k[9:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[49:])), 4) for k in bench.STAT_NAMES[49:]}, "work": {k: d[k] for k in bench.STAT_NAMES[11:23]}}
+           "share": {k[4:]: round(d[k] / max(1, d["cyc_total"]), 4) for k in bench.STAT_NAMES[:10] + bench.STAT_NAMES[23:40]}, "phase": {k[3:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[40:49])), 4) for k in bench.STAT_NAMES[40:49]}, "me_stage": {k[9:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[49:])), 4) for k in bench.STAT_NAMES[49:]}, "work": {k: d[k] for k in bench.STAT_NAMES[11:23]},
+           "search_phase_mcycles": {n: round(d["x_" + n] / 1e6) for n in SEARCH_PHASE_NAMES}}
     if args.trace:
         n = L.tb_rdo_batch_trace(b, None, 0)
         tr = np.zeros(n, [(k, np.int32) for k in ("frame", "row", "col", "cta")] + [("t_start", np.uint64), ("t_end", np.uint64)])
