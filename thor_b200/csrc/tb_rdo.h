@@ -720,7 +720,8 @@ template <class S, class B> struct Rdo {
   // mode_decision_rdo :1835-2120
   // ---------------------------------------------------------------------------------------------------------------
   // candidate indices in the reference's evaluation order after skip (k) and merge (num_skip + k * max_tb + tb): inter (IDX_INTER + (reference,
-  // partition) * (max_tb + 1) + tb_param + 1), bipred (IDX_BIPRED + tb_param, then the joint search of B frames), intra (IDX_INTRA + tb_param)
+  // partition) * (max_tb + 1) + tb_param + 1), bipred (IDX_BIPRED + tb_param, then the joint search of B frames), intra (with intra_rdo IDX_INTRA +
+  // intra_mode * max_tb + tb_param, the item of the intra-mode search; else IDX_INTRA + tb_param)
   enum { IDX_INTER = 64, IDX_BIPRED = IDX_INTER + TB_RDO_MAX_REF * 4 * 3, IDX_INTRA = IDX_BIPRED + 8 };
 
   TBR_HD void cand_group_begin() { loc_idx = 0x7fffffff; loc_cost = MAX_U32; loc_worst = 0; loc_bestc = MAX_U32; }
@@ -753,13 +754,15 @@ template <class S, class B> struct Rdo {
   TBR_HD static void set_from_ipred(Cand &c, const IPred &p, int idx) {
     c.skip_idx = idx; c.ref_idx0 = p.ref_idx0; c.ref_idx1 = p.ref_idx1; c.mv0[0] = p.mv0; c.mv1[0] = p.mv1; c.dir = p.bipred_flag;
   }
-  // one item of the intra-mode search (:2080-2097 with intra_rdo, else search_intra_prediction_params): the warp keeps its best (cost, k)
-  TBR_HD TBR_NI void intra_search_item(BlockInfo &bi, Cand &t, int k, uint32_t *best_cost, int *best_k) {
+  // item d (in the order the warps draw them) of the intra-mode search.  With intra_rdo (:2080-2097) the items are the (intra mode, tb_param) pairs,
+  // and pair k = (k / max_tb, k % max_tb) is the intra RD candidate of index IDX_INTRA + k (see mode_decision_rdo).  The pairs of tb_param 1 come
+  // first: they predict and transform four sub-blocks per plane one after another, so they are the longest, and the section should not end on one
+  // that started late.  Without intra_rdo: search_intra_prediction_params, and the warp keeps the mode it chose in (best_cost, best_k)
+  TBR_HD TBR_NI void intra_search_item(BlockInfo &bi, Cand &t, int d, uint32_t *best_cost, int *best_k) {
     if (F.intra_rdo) {
-      t.intra_mode = k / bi.max_tb; t.tb_param = k % bi.max_tb; t.mode = MODE_INTRA;
-      const int nbits = encode_block(bi, t);
-      const uint32_t cost = cost_calc(bi, bi.size, bi.size, nbits);
-      if (cost < *best_cost || (cost == *best_cost && k < *best_k)) { *best_cost = cost; *best_k = k; }
+      const int nm = F.num_intra_modes;
+      t.mode = MODE_INTRA; t.intra_mode = d % nm; t.tb_param = bi.max_tb - 1 - d / nm;
+      eval_cand(bi, t, bi.size, bi.size, IDX_INTRA + t.intra_mode * bi.max_tb + t.tb_param, false);
     } else {
       int mode;
       search_intra(bi, &mode);
@@ -782,13 +785,15 @@ template <class S, class B> struct Rdo {
   }
 
   // mode_decision_rdo :1835-2120.  The candidates in the reference's order: skip, merge x tb_param, inter (reference x partition x tb_param), bipred,
-  // the joint bipred of B frames, intra x tb_param; the warps deal them round robin by their position in the group.
+  // the joint bipred of B frames, intra x tb_param; the warps deal them round robin by their position in the group.  With intra_rdo the
+  // intra-mode search encodes every (intra mode, tb_param) with full RD, and those items are the intra candidates: the reference's second encode of
+  // the chosen mode (:2102-2113) repeats items of the search and is not run again (the argument is at the end of this function).
   // Square blocks of inter frames at encoder_speed 0 on more than one warp OVERLAP the sections that do not depend on each other instead:
   //   the references' motion searches run one warp per reference, and nothing else runs beside them;
   //   then warp 0 runs the bi-prediction chain (every search depends on the previous one) and evaluates its candidates, while the others draw the
   //   inter candidates (one draw = the tb_param variants of one prediction) from a shared counter;
-  //   after a barrier every warp draws the items of the intra-mode search, and the candidate lists the chain extends are copied to the other
-  //   warps' replicas.
+  //   after a barrier every warp draws the items of the intra-mode search (with intra_rdo, the intra candidates), and the candidate lists the
+  //   chain extends are copied to the other warps' replicas.
   // The RD loop is bound by instruction delivery: warps that run different code at the same time slow each other down (searches beside the
   // intra-mode search take about 1.5 times the cycles of searches alone), while a warp waiting at a barrier fetches nothing.  So the intra-mode search,
   // which no search and no inter candidate needs, runs neither beside the searches nor beside the chain, but in a section of its own.
@@ -881,7 +886,7 @@ template <class S, class B> struct Rdo {
         be.mark(PH_INTER_CAND);
         if (overlap) {  // the intra-mode search, once the chain and the inter candidates are done
           be.cta_sync();
-          for (int k; (k = be.next(1)) < n_isearch;) intra_search_item(bi, t, k, &my_icost, &my_ik);
+          for (int d; (d = be.next(1)) < n_isearch;) intra_search_item(bi, t, d, &my_icost, &my_ik);
           be.mark(PH_INTRA_SEARCH);
         }
         {
@@ -901,14 +906,23 @@ template <class S, class B> struct Rdo {
       }
       if (do_intra) {
         if (!overlap) {
-          for (int k = 0; k < n_isearch; k++)
-            if (be.mine(k)) intra_search_item(bi, t, k, &my_icost, &my_ik);
+          for (int d = 0; d < n_isearch; d++)
+            if (be.mine(d)) intra_search_item(bi, t, d, &my_icost, &my_ik);
           be.mark(PH_INTRA_SEARCH);
         }
-        be.reduce_best(&my_icost, &my_ik);
-        t.mode = MODE_INTRA; t.intra_mode = my_icost == MAX_U32 ? 0 : my_ik / bi.max_tb;
-        if (overlap) pos = 0;  // the overlapped schedule deals only the intra candidates by position
-        eval_tbs(bi, t, 0, IDX_INTRA, false, &pos, false);
+        // With intra_rdo the items of the search were the intra candidates.  The reference encodes (mode, tb_param) for every pair, keeps the mode
+        // of the first strictly smallest cost, then encodes that mode again for every tb_param (:2078-2113), on the same inputs.  Let k* be the
+        // first item of smallest cost c* and m* = k* / max_tb: the items of m* before k* cost more than c*, so its second pass picks
+        // tb_param k* % max_tb, and the reference's intra candidate is item k* with cost c*.  Every other item costs more, or costs c* with a
+        // larger k, so under min (cost, index) with index IDX_INTRA + k it loses to k* and beats nothing k* does not beat; IDX_INTRA + k is above
+        // every other candidate's index, so k* wins only with a strictly smaller cost, as in the reference.  The index must be IDX_INTRA + k, not
+        // IDX_INTRA + tb_param: then an item of another mode with the same cost (flat content) could win and code the wrong intra mode.
+        if (!F.intra_rdo) {  // search_intra chose the mode by SAD: its tb_param candidates
+          be.reduce_best(&my_icost, &my_ik);
+          t.mode = MODE_INTRA; t.intra_mode = my_ik / bi.max_tb;
+          if (overlap) pos = 0;  // the overlapped schedule deals only the intra candidates by position
+          eval_tbs(bi, t, 0, IDX_INTRA, false, &pos, false);
+        }
       }
     }
     const uint32_t cost = cand_group_end(bi, owner);
