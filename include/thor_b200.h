@@ -243,7 +243,7 @@ int tb_interpolate_frames(tb_frame_t *out, const tb_frame_t *ref0, const tb_fram
  * find_block_contexts common/common_block.c:283-303) for EVERY super block of one frame on the GPU (one CTA works on one super block at a time), super
  * blocks in a wavefront (left, up-left, up, up-right dependencies), and returns the decisions.  The host then only serialises them
  * (write_super_mode / write_block of the reference's own bit writer: thor_b200/csrc/tb_rdo_shim.c is that binding).
- * Supported: 4:2:0, sync = 0, qmtx = 0, interp_ref != 2, max_delta_qp = 0, bitrate = 0 (every BASELINE.json configuration);
+ * Supported: 4:2:0 at internal bit depth 8, 10 or 12, sync = 0, qmtx = 0, interp_ref != 2, max_delta_qp = 0, bitrate = 0 (every BASELINE.json configuration);
  * anything else returns TB_ERR_ARG and the binding falls back to the reference's host loop over the per-call drop-in kernels. */
 typedef struct { int16_t x, y; } tb_mv_t; /* mv_t, common/types.h:132-136 */
 typedef struct { /* per 4x4 luma block: the part of deblock_data_t (common/types.h:178-187) the RD loop and the in-loop filters read */

@@ -52,7 +52,7 @@ static const uint8_t orc_tc_table[56] = {0,  0,  1,  1,  2,  3,  4,  5,  6,  7, 
                                          17, 18, 20, 22, 24, 26, 28, 30, 32, 36, 40, 44, 48,  52,  56,  60,  64,  68,  72,
                                          80, 88, 96, 104, 112, 128, 144, 152, 160, 168, 176, 184, 192, 200, 208, 216, 224, 232};
 
-/* ---- a10: forward transform.  common/transform.c:245-308 (C path; int16 intermediates) ---- */
+/* ---- a10: forward transform.  common/transform.c:245-308 (C path; int16 intermediates), box sum as in transform_simd ---- */
 void orc_transform(const int16_t *block, int16_t *coeff, int size, int fast, int bitdepth) {
   static int16_t tmp[32][32], tmp2[32 * 32];
   const int16_t *in = block;
@@ -60,13 +60,19 @@ void orc_transform(const int16_t *block, int16_t *coeff, int size, int fast, int
   if (size > (32 >> fast)) {
     size1 = 32 >> fast;
     scale = size / size1;
+    /* The box sum is formed as the encoder's transform_simd forms it.  64x64 and 128x128 with `fast` saturate to [-16384, 16383] after every
+       addition (common/common_kernels.c:1524-1529).  The 2x2 sums of 32x32 with `fast` (:1501-1503) and the sums of 64x64 and 128x128 without
+       it (:1544-1549) wrap in int16.  The C transform saturates everywhere (common/transform.c:261-278).  The two rules differ only when a
+       partial sum leaves [-16384, 16383]: 4 residuals never do (4 x 4095 = 16380), and 16 residuals only above 10 bits (16 x 1023 = 16368),
+       so only 128x128 without `fast` at 12 bits tells them apart. */
+    const int sat = fast && size >= 64;
     for (int i = 0; i < size1; i++)
       for (int j = 0; j < size1; j++) {
         int16_t sum = 0;
         for (int m = 0; m < scale; m++)
           for (int n = 0; n < scale; n++) {
             int v = sum + block[(i * scale + m) * size + j * scale + n];
-            sum = (int16_t)(v < -16384 ? -16384 : v > 16383 ? 16383 : v);
+            sum = (int16_t)(!sat ? v : v < -16384 ? -16384 : v > 16383 ? 16383 : v); /* !sat: modulo 2^16 */
           }
         tmp2[i * size1 + j] = sum;
       }

@@ -93,6 +93,14 @@ def rand_plane(rng, h, w, bitdepth, hbd, smooth=False):
     return a
 
 
+def full_scale_planes(h, w, maxv):
+    """reconstructions whose intra neighbours sit at 0 and 2^bd-1: uniform, and stripes that put one of the top row and left column at 2^bd-1 and
+    alternate the other (the planar pre-filter's int16 input reaches 8 (2^bd-1), 32760 at 12 bits)"""
+    yy, xx = np.mgrid[0:h, 0:w]
+    return {"max": np.full((h, w), maxv), "zero": np.zeros((h, w), int), "odd rows": (yy % 2) * maxv, "even rows": (1 - yy % 2) * maxv,
+            "odd cols": (xx % 2) * maxv, "even cols": (1 - xx % 2) * maxv}
+
+
 def rdo_hostcheck():
     """oracle/librdo_hostcheck.so: tb_rdo.h over the plain-C oracle on the CPU (built by `make -C oracle port`, no reference sources needed).  It
     exports tb_rdo_encode_frame like libthor_b200.so, so it is loaded through its own handle and never RTLD_GLOBAL."""

@@ -7,6 +7,8 @@ SURVEY §8c.3.  The cases (CASES):
                        hierarchical B frames with interpolated reference and bipred)
   hdb_hard_q4_10bit    rdo_jobs_hdb_hard_q4_10bit.xz: 5 frames of 128x136 10-bit HDB at qp 4 on tests/test_rdo_matrix.py:hard_yuv (large
                        coefficients, saturated samples, local motion)
+  hdb_q51_12bit        rdo_jobs_hdb_q51_12bit.xz: 3 frames of 128x136 12-bit HDB at qp 51 on synth_yuv (an unsplit 128x128 block in each, one
+                       of them an intra block whose transform's box sum wraps in int16)
 Run in the development container (needs /root/reference compiled into oracle/_ref):  python tests/golden/make_golden_rdo.py [case ...]"""
 import lzma
 import os
@@ -23,6 +25,7 @@ CASES = {
     # name: (flags, width, height, frames, qp, bitdepth, clip writer name, output file)
     "hdb_128x136": (HDB + ["-cdef", "0"], 128, 136, 9, 32, 8, "synth", "rdo_jobs_hdb_128x136.xz"),
     "hdb_hard_q4_10bit": (HDB + ["-cdef", "0"], 128, 136, 5, 4, 10, "hard", "rdo_jobs_hdb_hard_q4_10bit.xz"),
+    "hdb_q51_12bit": (HDB + ["-cdef", "0"], 128, 136, 3, 51, 12, "synth", "rdo_jobs_hdb_q51_12bit.xz"),
 }
 
 

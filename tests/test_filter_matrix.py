@@ -10,7 +10,8 @@ tb_cdef_search_mse, tb_clpf_frame, tb_clpf_detect_frame and tb_interpolate_frame
             reconstruction and block state (the committed golden RD-loop jobs, and two captured cases of tests/test_rdo_matrix.py).
 
 The geometries reach what 64-multiple widths do not: partial 64x64 CDEF and CLPF filter blocks in both directions, chroma planes 4 samples wider
-than a multiple of 8, a 1-level and a 4-level interpolation pyramid with odd-sized levels, and the only large 10-bit case."""
+than a multiple of 8, a 1-level and a 4-level interpolation pyramid with odd-sized levels, and the only large 10-bit case.  Two geometries also run
+at 12 bits, where deblocking's tc is used unshifted and the CDEF and CLPF strengths and thresholds shift by 4."""
 import ctypes as C
 import math
 
@@ -29,10 +30,10 @@ needs_ref = pytest.mark.skipif(not HAVE_REF, reason="oracle/_ref not built")
 GEOMS = [
     # w     h     bit depths  why
     (64,   64,   (8, 10)),   # one CDEF block, one CLPF block at 64 and 128; a 2-level pyramid
-    (200,  136,  (8, 10)),   # partial filter blocks in both directions; chroma width 100 (4 mod 8, 4 mod 16)
+    (200,  136,  (8, 10, 12)),   # partial filter blocks in both directions; chroma width 100 (4 mod 8, 4 mod 16)
     (136,  200,  (8, 10)),   # the same, in portrait
     (240,  120,  (8, 10)),   # partial in width, luma width a multiple of 16 (no CDEF-search chroma quirk); a 2-level pyramid
-    (424,  264,  (8, 10)),   # a 4-level pyramid whose deepest level is 53x33
+    (424,  264,  (8, 10, 12)),   # a 4-level pyramid whose deepest level is 53x33
     (1920, 1080, (10,)),     # the only large high-bit-depth case
 ]
 CASES = [(w, h, bd) for w, h, bds in GEOMS for bd in bds]
@@ -703,7 +704,7 @@ def run_chain(tb, jobs, seed):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", ["hdb_128x136", "hdb_hard_q4_10bit"])
+@pytest.mark.parametrize("case", ["hdb_128x136", "hdb_hard_q4_10bit", "hdb_q51_12bit"])
 def test_filter_chain_on_golden_rdo_jobs(tb, tmp_path, case):
     from test_rdo_jobs import golden_jobs
     from thor_b200 import rdo_jobs as RJ

@@ -4,12 +4,12 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from _libs import oracle, ref, aligned, P, sdt, sfx, rand_plane
+from _libs import oracle, ref, aligned, P, sdt, sfx, rand_plane, full_scale_planes
 from _refstructs import Frame as HFrame, random_blkinfo
 
 pytestmark = pytest.mark.gpu
 O = oracle()
-BD = [(0, 8), (1, 10)]
+BD = [(0, 8), (1, 10), (1, 12)]
 
 
 @pytest.fixture(scope="module")
@@ -90,7 +90,7 @@ def test_dropin_interp_avg(tb, hbd, bd):
         assert (o0 == o1).all()
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 10, 12])
 def test_dropin_transform_quant(tb, bd):
     rng = np.random.default_rng(103)
     L = tb.lib
@@ -207,16 +207,17 @@ def test_cfl(tb, hbd, bd):
     rng = np.random.default_rng(105)
     s = sfx(hbd)
     hit = 0
+    ns = 1 << max(0, bd - 10)  # noise grows with the remap threshold above 10 bits (tests/test_oracle_vs_ref.py::test_cfl)
     for n in (8, 16, 32, 64):
         for trial in range(12):
             y = rand_plane(rng, n, n, bd, hbd, smooth=True)
             ry = aligned((n, n + 8), sdt(hbd))
-            ry[...] = np.clip(np.pad(y.astype(int), ((0, 0), (0, 8)), mode="edge") + rng.integers(-40, 41, (n, n + 8)) * (trial % 3), 0, (1 << bd) - 1)
+            ry[...] = np.clip(np.pad(y.astype(int), ((0, 0), (0, 8)), mode="edge") + rng.integers(-40, 41, (n, n + 8)) * (trial % 3) * ns, 0, (1 << bd) - 1)
             k = float(rng.uniform(-1.5, 1.5))
             ys = y.astype(int).reshape(n // 2, 2, n // 2, 2).sum(axis=(1, 3)) // 4
             u0 = aligned((n // 2, n // 2), sdt(hbd)); v0 = aligned((n // 2, n // 2), sdt(hbd))
-            u0[...] = np.clip(ys * k + (1 << (bd - 1)) * (1 - k) + rng.integers(-3, 4, ys.shape), 0, (1 << bd) - 1)
-            v0[...] = np.clip(ys * -k + (1 << (bd - 1)) * (1 + k) + rng.integers(-30, 31, ys.shape), 0, (1 << bd) - 1)
+            u0[...] = np.clip(ys * k + (1 << (bd - 1)) * (1 - k) + rng.integers(-3, 4, ys.shape) * ns, 0, (1 << bd) - 1)
+            v0[...] = np.clip(ys * -k + (1 << (bd - 1)) * (1 + k) + rng.integers(-30, 31, ys.shape) * ns, 0, (1 << bd) - 1)
             u1 = aligned(u0.shape, sdt(hbd)); u1[...] = u0; v1 = aligned(v0.shape, sdt(hbd)); v1[...] = v0
             ub = u0.copy()
             getattr(O, "orc_cfl_" + s)(P(y), P(u0), P(v0), P(ry), n, n, n + 8, 1, bd)
@@ -522,6 +523,67 @@ def test_batch_txfm_chain(tb, hbd, bd):
     assert 0 < ncbp < n
 
 
+def full_scale_blocks(bd, hbd, n=128):
+    """(name, orig, pred) n x n pairs whose residual is +-(2^bd-1): constant of either sign, 8x8 cells and single samples of alternating sign"""
+    maxv = (1 << bd) - 1
+    yy, xx = np.mgrid[0:n, 0:n]
+    out = []
+    for name, o in (("max - 0", np.ones((n, n), int)), ("0 - max", np.zeros((n, n), int)), ("cells", (yy // 8 + xx // 8) % 2), ("dots", (yy + xx) % 2)):
+        org = aligned((n, n), sdt(hbd)); prd = aligned((n, n), sdt(hbd))
+        org[...] = o * maxv; prd[...] = (1 - o) * maxv
+        out.append((name, org, prd))
+    return out
+
+
+@pytest.mark.parametrize("hbd,bd", BD)
+def test_batch_txfm_chain_full_scale(tb, hbd, bd):
+    """the chain on residuals of +-(2^bd-1) at every size, qp and fast flag, where the int16 intermediates have the least headroom: at 12 bits
+    the box sums of 128x128 without fast wrap in int16 and those with fast saturate (common/common_kernels.c:1519-1551)"""
+    s = sfx(hbd)
+    esz = 2 if hbd else 1
+    pats = full_scale_blocks(bd, hbd)
+    d_org = [tb.DevBuf.from_array(o) for _, o, _ in pats]; d_prd = [tb.DevBuf.from_array(p) for _, _, p in pats]
+    meta = []
+    for k in range(len(pats)):
+        for size in (4, 8, 16, 32, 64, 128):
+            for qp in range(52):
+                for fast in (0, 1):
+                    meta.append((k, size, qp, (qp + size + k) % 4, fast))
+    n = len(meta)
+    recofs = np.cumsum([0] + [m[1] * m[1] for m in meta])
+    recbuf = tb.DevBuf(int(recofs[-1]) * esz); cqbuf = tb.DevBuf(n * 512)
+    items = np.zeros(n, tb.TXFM_ITEM)
+    for i, (k, size, qp, typ, fast) in enumerate(meta):
+        items[i] = (d_org[k].ptr, d_prd[k].ptr, recbuf.ptr + int(recofs[i]) * esz, cqbuf.ptr + i * 512, 128, 128, size, size, qp, typ, fast | tb.TXFM_BITS)
+    d_items = tb.DevBuf.from_array(items); d_out = tb.DevBuf(16 * n)
+    tb.check(tb.lib.tb_txfm_chain_batch(d_items.ptr, n, esz, bd, d_out.ptr))
+    res = d_out.download(tb.TXFM_RESULT, n)
+    rec = recbuf.download(sdt(hbd), (int(recofs[-1]),))
+    cq = cqbuf.download(np.int16, (n, 256))
+    bad = []
+    for i, (k, size, qp, typ, fast) in enumerate(meta):
+        name, org, prd = pats[k]
+        q = min(size, 16)
+        blk = aligned((size, size), np.int16); cf = aligned((size, size), np.int16, fill=0); cq0 = aligned((q * q,), np.int16, fill=0)
+        getattr(O, "orc_residual_" + s)(P(blk), P(prd), P(org), size, 128, 128)
+        O.orc_transform(P(blk), P(cf), size, fast, bd)
+        cbp = O.orc_quantize(P(cf), P(cq0), qp, size, typ, None)
+        want = aligned((size, size), sdt(hbd))
+        if cbp:
+            rc = aligned((size, size), np.int16, fill=0); rb = aligned((size, size), np.int16)
+            O.orc_dequantize(P(cq0), P(rc), qp, size, None)
+            O.orc_inverse_transform(P(rc), P(rb), size, bd)
+            getattr(O, "orc_reconstruct_" + s)(P(rb), P(prd), P(want), size, 128, size, bd)
+        else:
+            want[...] = prd[:size, :size]
+        ssd = getattr(O, "orc_ssd_" + s)(P(org), P(want), 128, size, size, size)
+        bits = O.orc_coeff_bits(P(cq0), size, typ) if cbp else 0
+        got = rec[recofs[i]:recofs[i] + size * size].reshape(size, size)
+        if not (int(res[i]["cbp"]) == cbp and (cq[i, :q * q] == cq0).all() and (got == want).all() and int(res[i]["ssd"]) == ssd and int(res[i]["bits"]) == bits):
+            bad.append((name, size, qp, typ, fast))
+    assert not bad, (len(bad), bad[:8])
+
+
 @pytest.mark.parametrize("hbd,bd", BD)
 def test_batch_intra(tb, hbd, bd):
     rng = np.random.default_rng(111)
@@ -554,6 +616,42 @@ def test_batch_intra(tb, hbd, bd):
         want = aligned((size, size), sdt(hbd))
         getattr(O, "orc_intra_pred_" + s)(P(left), P(top), int(tl[0]), ypos, xpos, size, P(want), size, mode, bd)
         assert (got[i, :size * size].reshape(size, size) == want).all(), (i, meta[i])
+
+
+@pytest.mark.parametrize("hbd,bd", BD)
+def test_batch_intra_full_scale_neighbours(tb, hbd, bd):
+    """every intra mode and size with neighbours at 0 and 2^bd-1, at the frame's edges and inside it, with and without the up-right and
+    down-left neighbours"""
+    s = sfx(hbd)
+    w, h = 192, 128
+    esz = 2 if hbd else 1
+    for name, v in full_scale_planes(h, w, (1 << bd) - 1).items():
+        f = HFrame(w, h, bd, hbd)
+        f.y[...] = v
+        drec = tb.Frame(w, h, esz)
+        drec.upload(f.y, f.u, f.v)
+        ptr, st = drec.plane(0)
+        meta = []
+        for size in (4, 8, 16, 32, 64):
+            for xpos, ypos in ((0, 0), (size, 0), (0, size), (size, size), (w - 2 * size, h - 2 * size)):
+                for mode in range(10):
+                    ur = int(ypos > 0 and xpos + size < w)
+                    dl = int(xpos > 0 and ypos + size < h and mode % 2 == 0)
+                    meta.append((size, xpos, ypos, mode, ur, dl))
+        n = len(meta)
+        items = np.zeros(n, tb.INTRA_ITEM)
+        out = tb.DevBuf(n * 64 * 64 * esz)
+        for i, (size, xpos, ypos, mode, ur, dl) in enumerate(meta):
+            items[i] = (ptr + (ypos * st + xpos) * esz, out.ptr + i * 64 * 64 * esz, st, xpos, ypos, size, mode, ur, dl)
+        d_items = tb.DevBuf.from_array(items)
+        tb.check(tb.lib.tb_intra_batch(d_items.ptr, n, esz, bd))
+        got = out.download(sdt(hbd), (n, 64 * 64))
+        for i, (size, xpos, ypos, mode, ur, dl) in enumerate(meta):
+            left = aligned((264,), sdt(hbd), fill=0); top = aligned((264,), sdt(hbd), fill=0); tl = aligned((1,), sdt(hbd), fill=0)
+            getattr(O, "orc_make_top_and_left_" + s)(P(left), P(top), P(tl), P(f.Y, f.origin(0) + ypos * f.sy + xpos), f.sy, None, 0, 0, 0, ypos, xpos, size, ur, dl, 0, bd)
+            want = aligned((size, size), sdt(hbd))
+            getattr(O, "orc_intra_pred_" + s)(P(left), P(top), int(tl[0]), ypos, xpos, size, P(want), size, mode, bd)
+            assert (got[i, :size * size].reshape(size, size) == want).all(), (name, meta[i])
 
 
 def run_filters(tb, rng, w, h, bd, hbd, qp=33):

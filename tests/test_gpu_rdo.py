@@ -27,8 +27,10 @@ def enc(exe, flags, w, h, n, tag, tmp, extra, env=None, qp=32):
 
 
 # qp and clip of the cases that do not encode synth_yuv at qp 32: low qp on 10-bit hard content (large coefficients, saturation), nearly everything
-# skipped (qp 51), cfl_inter, encoder speed 1 on a frame narrower than two super blocks
-CLIPS = {"hdb_10bit_q4_hard": (4, hard_yuv), "hdb_8bit_q51": (51, synth_yuv), "hdb_8bit_cfl_inter_hard": (22, hard_yuv), "hdb_8bit_speed1_rect_hard": (8, hard_yuv)}
+# skipped (qp 51), cfl_inter, encoder speed 1 on a frame narrower than two super blocks, 12 bits at qp 51 (a 128x128 intra block whose transform's
+# box sum wraps in int16)
+CLIPS = {"hdb_10bit_q4_hard": (4, hard_yuv), "hdb_8bit_q51": (51, synth_yuv), "hdb_8bit_cfl_inter_hard": (22, hard_yuv), "hdb_8bit_speed1_rect_hard": (8, hard_yuv),
+         "hdb_12bit_q51": (51, synth_yuv)}
 
 
 @pytest.mark.gpu
@@ -44,11 +46,12 @@ CLIPS = {"hdb_10bit_q4_hard": (4, hard_yuv), "hdb_8bit_q51": (51, synth_yuv), "h
     ("hdb_8bit_q51", HDB + ["-cdef", "0"], 128, 136, 9, (), True),
     ("hdb_8bit_cfl_inter_hard", HDB + ["-cdef", "0", "-enable_cfl_inter", "1"], 128, 136, 5, (), True),
     ("hdb_8bit_speed1_rect_hard", HDB + ["-cdef", "0", "-encoder_speed", "1"], 200, 72, 5, (), True),
+    ("hdb_12bit_q51", HDB + ["-cdef", "0"], 128, 136, 5, ("-bitdepth", "12", "-input_bitdepth", "12"), True),
 ])
 def test_device_rd_loop_encode_is_bit_exact(tmp_path, name, flags, w, h, n, extra, decode):
     tmp = str(tmp_path)
     qp, make_clip = CLIPS.get(name, (32, synth_yuv))
-    make_clip(os.path.join(tmp, "in.yuv"), w, h, n, 10 if "10bit" in name else 8)
+    make_clip(os.path.join(tmp, "in.yuv"), w, h, n, 12 if "12bit" in name else 10 if "10bit" in name else 8)
     bit_ref, rec_ref, _, _ = enc("Thorenc", flags, w, h, n, "ref", tmp, extra, qp=qp)
     bit, rec, err, bitfile = enc("Thorenc_b200_rdo", flags, w, h, n, "gpu", tmp, extra, {"TB_RDO_STATS": "1"}, qp=qp)
     assert "frames decided by tb_rdo_encode_frame: %d," % n in err, err[-800:]   # every frame went through the device RD loop (no host-loop frames)

@@ -3,13 +3,13 @@ built from /root/reference by oracle/Makefile).  CPU only.  Skipped when oracle/
 import ctypes as C
 import numpy as np
 import pytest
-from _libs import oracle, ref, ref_enc, aligned, P, sdt, sfx, rand_plane
+from _libs import oracle, ref, ref_enc, aligned, P, sdt, sfx, rand_plane, full_scale_planes
 from _refstructs import Frame, random_blkinfo, CdefStrengths, Mv
 
 pytestmark = pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 O = oracle()
 R = ref()
-BD = [(0, 8), (1, 10)]
+BD = [(0, 8), (1, 10), (1, 12)]
 
 
 def test_tables():
@@ -152,7 +152,7 @@ def test_clip_mv_and_bits():
         assert E.ref_quote_mv_bits_lbd(dy, dx) == O.orc_quote_mv_bits(dy, dx)
 
 
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 10, 12])
 def test_transform_chain(bd):
     rng = np.random.default_rng(5)
     E = ref_enc(0)
@@ -193,6 +193,61 @@ def test_transform_chain(bd):
             R.inverse_transform_simd(P(r0), P(b1), size, bd)
             assert O.orc_check_nz_area(P(r0), size) == R.check_nz_area(P(r0), size)
             assert (b0 == b1).all()
+
+
+def box_sum_blocks(rng, size, bd):
+    """64x64 and 128x128 residual blocks whose box sums cross +-16384 by small and large amounts at 12 bits: constant blocks at +-(2^bd-1) and
+    at +-1025 / -1026 (16 samples sum to 16400 / -16416), checkerboards of 8x8 cells at +-(2^bd-1) and +-2048, sample checkerboards of the same
+    amplitudes, cells of random sign near full scale, and uniform noise at full scale"""
+    lim = (1 << bd) - 1
+    yy, xx = np.mgrid[0:size, 0:size]
+    cell = np.where((yy // 8 + xx // 8) % 2, 1, -1)
+    dot = np.where((yy + xx) % 2, 1, -1)
+    signs = np.kron(rng.choice([-1, 1], (size // 8, size // 8)), np.ones((8, 8), int))
+    pats = {"+max": np.full((size, size), lim), "-max": np.full((size, size), -lim), "+1025": np.full((size, size), min(1025, lim)),
+            "-1026": np.full((size, size), -min(1026, lim)),
+            "cells max": cell * lim, "cells 2048": cell * min(2048, lim), "dots max": dot * lim, "dots 2048": dot * min(2048, lim),
+            "cells near max": signs * rng.integers(lim - 200, lim + 1, (size, size)), "noise": rng.integers(-lim, lim + 1, (size, size))}
+    for name, v in pats.items():
+        blk = aligned((size, size), np.int16)
+        blk[...] = v
+        yield name, blk
+
+
+@pytest.mark.parametrize("bd", [10, 12])
+@pytest.mark.parametrize("size", [64, 128])
+def test_transform_box_sum_against_transform_simd(bd, size):
+    """transform_simd's box sum (common/common_kernels.c:1519-1551): 64x64 and 128x128 without fast wrap in int16, with fast they saturate.
+    The wrapping sums leave [-16384, 16383] only for 128x128 at 12 bits (16 x 4095 = 65520).  The coefficients are then quantised, dequantised
+    and inverse transformed at every qp and coefficient type; 10 bits is the control where no wrapping sum leaves the range"""
+    rng = np.random.default_rng(24)
+    E = ref_enc(0)
+    q = 16
+    for fast in (0, 1):
+        scale, crossed = size // (32 >> fast), False
+        for name, blk in box_sum_blocks(rng, size, bd):
+            box = blk.astype(np.int64).reshape(size // scale, scale, size // scale, scale).sum(axis=(1, 3))
+            crossed |= bool(((box < -16384) | (box > 16383)).any())
+            c0 = aligned((size, size), np.int16, fill=0); c1 = aligned((size, size), np.int16, fill=0)
+            O.orc_transform(P(blk), P(c0), size, fast, bd)
+            R.transform_simd(P(blk), P(c1), size, fast, bd)
+            assert (c0[:q, :q] == c1[:q, :q]).all(), (size, fast, name)
+            for qp in range(52):
+                for typ in range(4):
+                    q0 = aligned((q * q,), np.int16, fill=0); q1 = aligned((q * q,), np.int16, fill=0)
+                    cb0 = O.orc_quantize(P(c0), P(q0), qp, size, typ, None)
+                    cb1 = E.ref_quantize_lbd(P(c0), P(q1), qp, size, typ, None)
+                    assert cb0 == cb1 and (q0 == q1).all(), (size, fast, name, qp, typ)
+                r0 = aligned((size, size), np.int16, fill=0); r1 = aligned((size, size), np.int16, fill=0)
+                O.orc_dequantize(P(q0), P(r0), qp, size, None)
+                R.dequantize_lbd(P(q1), P(r1), qp, size, None)
+                assert (r0 == r1).all(), (size, fast, name, qp)
+                b0 = aligned((size, size), np.int16, fill=0); b1 = aligned((size, size), np.int16, fill=0)
+                O.orc_inverse_transform(P(r0), P(b0), size, bd)
+                R.inverse_transform(P(r1), P(b1), size, bd)
+                assert (b0 == b1).all(), (size, fast, name, qp)
+        # the patterns reach the int16 bound wherever scale^2 full-scale residuals can: 128x128 without fast only at 12 bits
+        assert crossed == (scale * scale * ((1 << bd) - 1) > 16383), (size, fast)
 
 
 def test_calc_cbp():
@@ -271,20 +326,52 @@ def test_intra(hbd, bd):
 
 
 @pytest.mark.parametrize("hbd,bd", BD)
+def test_intra_full_scale_neighbours(hbd, bd):
+    """every intra mode and size with neighbours at 0 and 2^bd-1 (the planar pre-filter's int16 input reaches 8 (2^bd-1), 32760 at 12 bits)"""
+    s = sfx(hbd)
+    dt = sdt(hbd)
+    W, H = 192, 128
+    for name, v in full_scale_planes(H + 8, W + 8, (1 << bd) - 1).items():
+        frame = aligned((H + 8, W + 8), dt)
+        frame[...] = v
+        rblock = aligned((130, 130), dt, fill=0)
+        for size in (4, 8, 16, 32, 64):
+            for xpos, ypos in ((0, 0), (size, 0), (0, size), (size, size), (W - 2 * size, H - 2 * size)):
+                base = (4 + ypos) * (W + 8) + 4 + xpos
+                ur, dl = int(ypos > 0 and xpos + size < W), int(xpos > 0 and ypos + size < H)
+                res = []
+                for lib, pre in ((O, "orc_"), (R, "")):
+                    left = aligned((2 * 128 + 8,), dt, fill=0); top = aligned((2 * 128 + 8,), dt, fill=0); tl = aligned((1,), dt, fill=0)
+                    getattr(lib, pre + "make_top_and_left_" + s)(P(left), P(top), P(tl), P(frame, base), W + 8, P(rblock, 131), 130, 0, 0, ypos, xpos, size, ur, dl, 0, bd)
+                    preds = []
+                    for mode in range(10):
+                        pb = aligned((size, size), dt, fill=0)
+                        fn = getattr(lib, "orc_intra_pred_" + s if lib is O else "get_intra_prediction_" + s)
+                        fn(P(left), P(top), int(tl[0]), ypos, xpos, size, P(pb), size, mode, bd)
+                        preds.append(pb.copy())
+                    res.append(preds)
+                for m in range(10):
+                    assert (res[0][m] == res[1][m]).all(), (name, size, xpos, ypos, m)
+
+
+@pytest.mark.parametrize("hbd,bd", BD)
 def test_cfl(hbd, bd):
     rng = np.random.default_rng(9)
     s = sfx(hbd)
     hit = 0
+    # the remap needs a mean squared luma residual above 64 << 2 (bd - 8) (common/common_block.c:361); the noise grows with it above 10 bits
+    ns = 1 << max(0, bd - 10)
     for n in (8, 16, 32, 64):
         for trial in range(40):
             y = rand_plane(rng, n, n, bd, hbd, smooth=True)
             ry = aligned((n, n + 8), sdt(hbd))
-            ry[...] = np.clip(y.astype(int)[:, :1] * 0 + np.pad(y.astype(int), ((0, 0), (0, 8)), mode="edge") + rng.integers(-40, 41, (n, n + 8)) * (trial % 3), 0, (1 << bd) - 1)
+            ry[...] = np.clip(y.astype(int)[:, :1] * 0 + np.pad(y.astype(int), ((0, 0), (0, 8)), mode="edge") + rng.integers(-40, 41, (n, n + 8)) * (trial % 3) * ns, 0,
+                              (1 << bd) - 1)
             k = float(rng.uniform(-1.5, 1.5))
             ys = y.astype(int).reshape(n // 2, 2, n // 2, 2).sum(axis=(1, 3)) // 4
             u0 = aligned((n // 2, n // 2), sdt(hbd)); v0 = aligned((n // 2, n // 2), sdt(hbd))
-            u0[...] = np.clip(ys * k + (1 << (bd - 1)) * (1 - k) + rng.integers(-3, 4, ys.shape), 0, (1 << bd) - 1)
-            v0[...] = np.clip(ys * -k + (1 << (bd - 1)) * (1 + k) + rng.integers(-30, 31, ys.shape), 0, (1 << bd) - 1)
+            u0[...] = np.clip(ys * k + (1 << (bd - 1)) * (1 - k) + rng.integers(-3, 4, ys.shape) * ns, 0, (1 << bd) - 1)
+            v0[...] = np.clip(ys * -k + (1 << (bd - 1)) * (1 + k) + rng.integers(-30, 31, ys.shape) * ns, 0, (1 << bd) - 1)
             u1, v1 = u0.copy(), v0.copy()
             u1 = aligned(u0.shape, sdt(hbd), fill=0); u1[...] = u0; v1 = aligned(v0.shape, sdt(hbd), fill=0); v1[...] = v0
             ub = u0.copy()
@@ -672,7 +759,7 @@ def test_coeff_bits():
     assert n > 1500
 
 
-@pytest.mark.parametrize("hbd,bd", [(0, 8), (1, 10)])
+@pytest.mark.parametrize("hbd,bd", BD)
 def test_motion_estimate_sync(hbd, bd):
     """a5 gap of round 1: motion_estimate_sync (enc/encode_block.c:713-796, -sync 1) restated in the oracle and pinned against the reference's file-static function
     through the trampoline.  (No CUDA form yet: the RD-loop binding leaves -sync 1 to the reference's own loop.)"""

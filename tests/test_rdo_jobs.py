@@ -82,8 +82,9 @@ def test_batched_rd_loop_equals_reference_decisions(tmp_path, name, flags, w, h,
 # ---- committed golden jobs (tests/golden/rdo_jobs_*.xz, generated from the reference by tests/golden/make_golden_rdo.py):
 #   hdb_128x136        9 frames of 128x136 HDB at qp 32 on smooth content (I, P, seven hierarchical B frames)
 #   hdb_hard_q4_10bit  5 frames of 128x136 10-bit HDB at qp 4 on tests/test_rdo_matrix.py:hard_yuv (large coefficients, saturated samples)
+#   hdb_q51_12bit      3 frames of 128x136 12-bit HDB at qp 51 on smooth content (an unsplit 128x128 block in every frame)
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-GOLDEN_FRAMES = {"hdb_128x136": 9, "hdb_hard_q4_10bit": 5}
+GOLDEN_FRAMES = {"hdb_128x136": 9, "hdb_hard_q4_10bit": 5, "hdb_q51_12bit": 3}
 
 
 def golden_module():
@@ -146,6 +147,11 @@ def test_hard_low_qp_golden_rdo_jobs_are_what_the_reference_writes_today(tmp_pat
     rederive(tmp_path, "hdb_hard_q4_10bit")
 
 
+@needs
+def test_12bit_golden_rdo_jobs_are_what_the_reference_writes_today(tmp_path):
+    rederive(tmp_path, "hdb_q51_12bit")
+
+
 @pytest.mark.parametrize("case", sorted(GOLDEN_FRAMES))
 def test_host_decisions_of_the_golden_jobs_code_alike_with_any_warp_count(tmp_path, case):
     """oracle/librdo_hostcheck.so (tb_rdo.h over the oracle; no reference needed) returns the reference's decisions on the committed jobs, and
@@ -184,4 +190,15 @@ def test_batched_rd_loop_on_the_hard_low_qp_golden_jobs(tmp_path):
     golden_jobs(str(tmp_path), "hdb_hard_q4_10bit")
     jobs = RJ.load_jobs(str(tmp_path))
     assert len(jobs) == 5 and all(j.hdr.bitdepth == 10 and j.hdr.qp <= 8 for j in jobs)
+    decide_and_check(jobs)
+
+
+@pytest.mark.gpu
+def test_batched_rd_loop_on_the_12bit_golden_jobs(tmp_path):
+    """the same on the 12-bit qp 51 fixture: every frame holds an unsplit 128x128 block, and the first frame's is an intra block whose transform's
+    box sum wraps in int16 (common/common_kernels.c:1544-1549)"""
+    from thor_b200 import rdo_jobs as RJ
+    golden_jobs(str(tmp_path), "hdb_q51_12bit")
+    jobs = RJ.load_jobs(str(tmp_path))
+    assert len(jobs) == 3 and all(j.hdr.bitdepth == 12 and (j.blk["size"] == 128).any() for j in jobs)
     decide_and_check(jobs)

@@ -2,14 +2,16 @@
 
 One table of cases (CASES) drives every test here:
   CPU  oracle/_ref/Thorenc_rdocheck with TB_RDO_VERIFY=1: every super block of every case, decided by thor_b200/csrc/tb_rdo.h over the plain-C
-       oracle and by the reference's process_block() on the same encoder state, must be identical; two cases also run with eight simulated warps.
+       oracle and by the reference's process_block() on the same encoder state, must be identical; four cases also run with eight simulated warps.
   GPU  every case captured with the reference (oracle/_ref/Thorenc_capture); all 8-bit frames of all cases decided in ONE tb_rdo_encode_frames()
-       launch, all 10-bit frames in a second one.  Frames of one launch differ in size, qp, speed and options.  Every frame must return the
-       reference's reconstruction, block state and cost per super block, and the leaf lists and coefficients that oracle/librdo_hostcheck.so
-       (tb_rdo.h over the oracle, itself checked against the reference first) returns for the same job: everything the bit writer reads.
+       launch, all 10-bit frames in a second one, all 12-bit frames in a third.  Frames of one launch differ in size, qp, speed and options.  Every
+       frame must return the reference's reconstruction, block state and cost per super block, and the leaf lists and coefficients that
+       oracle/librdo_hostcheck.so (tb_rdo.h over the oracle, itself checked against the reference first) returns for the same job: everything the
+       bit writer reads.
 The cases reach what qp 32 on smooth content does not: large coefficients and saturation in the transform chain (low qp), frames that are nearly
 all skipped (qp 51), samples at 0 and 2^bd-1 in prediction, bipred average and reconstruction, intra blocks in inter frames (a scene cut), local
-motion, cfl_inter, encoder speeds 1 and 3, block contexts off, no tb split, intra_rdo 0, no early skip and two references."""
+motion, cfl_inter, encoder speeds 1 and 3, block contexts off, no tb split, intra_rdo 0, no early skip, two references, and 12 bits, where the box
+sum of a 128x128 transform can wrap in int16 (hdb_q51_12 codes an unsplit 128x128 block in every frame)."""
 import ctypes as C
 import os
 import re
@@ -69,6 +71,11 @@ CASES = [
     ("max_ref2",         HDB0 + ["-max_num_ref", "2"],                                 128, 136, 9, 32, 8,  "synth"),
     ("no_early_skip",    HDB0 + ["-early_skip_thr", "0"],                              128, 136, 9, 32, 8,  "synth"),
     ("ldb_q45_hard",     LDB,                                                          256, 136, 4, 45, 8,  "hard"),
+    # 12 bits: box sums of 16 residuals leave int16 (128x128 transforms wrap), the inverse transform's second stage can saturate
+    ("hdb_q51_12",       HDB0,                                                         128, 136, 5, 51, 12, "synth"),
+    ("hdb_q4_hard_12",   HDB0,                                                         128, 136, 5, 4,  12, "hard"),
+    ("hdb_q32_hard_12",  HDB0,                                                         128, 136, 5, 32, 12, "hard"),
+    ("speed1_hard_12",   HDB0 + ["-encoder_speed", "1"],                               128, 136, 5, 45, 12, "hard"),
 ]
 BY_NAME = {c[0]: c for c in CASES}
 
@@ -107,7 +114,7 @@ def test_every_super_block_matches_reference_process_block(tmp_path, case):
 
 
 @needs_check
-@pytest.mark.parametrize("name", ["cfl_inter_hard", "hdb_q4_hard_10"])
+@pytest.mark.parametrize("name", ["cfl_inter_hard", "hdb_q4_hard_10", "hdb_q51_12", "speed1_hard_12"])
 def test_overlapped_decision_with_the_device_warp_count(tmp_path, name):
     """the device decides with eight warps per CTA; host threads stand in for them (TBR_HOST_WARPS), see tests/test_rdo_host.py"""
     verify(str(tmp_path), BY_NAME[name], {"TBR_HOST_WARPS": "8"})
@@ -138,6 +145,7 @@ def matrix_jobs(tmp_path_factory):
         d = str(tmp_path_factory.mktemp(name))
         jobdir = capture(d, flags, w, h, n, bd, qp, CONTENT[content])
         return name, (jobdir, RJ.load_jobs(jobdir))
+    tmp_path_factory.getbasetemp()  # created lazily: threads that create it at once get different ones, and mktemp then refuses the name
     with ThreadPoolExecutor(min(8, os.cpu_count() or 1)) as ex:
         return dict(ex.map(one, CASES))
 
@@ -165,7 +173,7 @@ def launches(matrix_jobs):
 
 @pytest.mark.gpu
 @needs_capture
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 10, 12])
 def test_matrix_in_one_launch_equals_reference_decisions(launches, bd):
     rc, hosts, err = launches(bd)
     assert rc == 0, err
@@ -176,7 +184,7 @@ def test_matrix_in_one_launch_equals_reference_decisions(launches, bd):
 
 @pytest.mark.gpu
 @needs_capture
-@pytest.mark.parametrize("bd", [8, 10])
+@pytest.mark.parametrize("bd", [8, 10, 12])
 def test_matrix_leaf_lists_and_coefficients_equal_host_decisions(launches, matrix_jobs, bd):
     import multiprocessing
     from concurrent.futures import ProcessPoolExecutor

@@ -1436,7 +1436,10 @@ __device__ void warp_fwd_transform(const int16_t *block, int bpitch, int size, i
   if (size > (32 >> fast)) { size1 = 32 >> fast; scale = size / size1; }
   const int l1 = ilog2(size1), qsize = min(size, 16);
   const int16_t *M = tab + dct_tab_ofs(l1);
-  // load (with box-sum down-scaling for large blocks, saturating like common/transform.c:261-278)
+  // load, with the box sum of large blocks formed as transform_simd forms it: 64x64 and 128x128 with `fast` saturate after every
+  // addition (common/common_kernels.c:1524-1529), every other box sum wraps in int16 (:1501-1503, :1544-1549).  The rules differ only
+  // for 128x128 without `fast` above 10 bits: no partial sum of at most 16 residuals of 10 bits or fewer leaves [-16384, 16383].
+  const bool sat = fast && size >= 64;
   for (int p = lane; p < size1 * size1; p += 32) {
     int i = p >> l1, j = p & (size1 - 1);
     int v;
@@ -1444,10 +1447,13 @@ __device__ void warp_fwd_transform(const int16_t *block, int bpitch, int size, i
     else {
       int sum = 0;
       for (int m = 0; m < scale; m++)
-        for (int n = 0; n < scale; n++) sum = iclip(sum + block[(i * scale + m) * bpitch + j * scale + n], -16384, 16383);
+        for (int n = 0; n < scale; n++) {
+          sum += block[(i * scale + m) * bpitch + j * scale + n];
+          if (sat) sum = iclip(sum, -16384, 16383);
+        }
       v = sum;
     }
-    sc.in[i * 33 + j] = (int16_t)v;
+    sc.in[i * 33 + j] = (int16_t)v;  // modulo 2^16
   }
   __syncwarp();
   const FwdRound R(ilog2(size), ilog2(scale), bitdepth);

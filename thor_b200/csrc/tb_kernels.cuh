@@ -320,8 +320,11 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
   const int l1 = ilog2(size1), qsize = min(size, 16), lq = ilog2(qsize);
   const int8_t *M1 = tab8 + dct_tab8_ofs(l1);
   const int mp1 = dct_tab8_pitch(l1);
-  // residual (enc/encode_block.c:162-171) fused with the box-sum load of the forward transform (common/transform.c:261-278:
-  // the sum saturates after every addition, rows outer / columns inner)
+  // residual (enc/encode_block.c:162-171) fused with the box-sum load of the forward transform, rows outer / columns inner, formed as
+  // transform_simd forms it: 64x64 and 128x128 with `fast` saturate to [-16384, 16383] after every addition (common/common_kernels.c:
+  // 1524-1529); the 2x2 sums of 32x32 with `fast` and 64x64, and the 4x4 sums of 128x128, wrap in int16 (:1501-1503, :1544-1549).
+  // The rules differ only for 128x128 without `fast` above 10 bits: a partial sum of 4 residuals stays within [-16384, 16383] at every
+  // bit depth (4 x 4095 = 16380), one of 16 residuals up to 10 bits (16 x 1023 = 16368).
   if (scale == 1) {
     for (int p = tid; p < (size1 * size1) >> 2; p += NT) {  // four samples per thread and step
       int i = p >> (l1 - 2), j = (p & ((size1 >> 2) - 1)) << 2;
@@ -330,7 +333,7 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
       load_row4<S>(pred + i * q.pstride + j, b);
       *(uint2 *)&sc.in[i * PI + j] = make_uint2(((uint32_t)(a[0] - b[0]) & 0xffffu) | ((uint32_t)(a[1] - b[1]) << 16), ((uint32_t)(a[2] - b[2]) & 0xffffu) | ((uint32_t)(a[3] - b[3]) << 16));
     }
-  } else if (scale == 4) {
+  } else if (scale == 4) {  // 128x128 (wraps) or 64x64 with `fast` (saturates)
     for (int p = tid; p < size1 * size1; p += NT) {
       int i = p >> l1, j = p & (size1 - 1), sum = 0;
       for (int m = 0; m < 4; m++) {
@@ -338,24 +341,24 @@ __device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth,
         load_row4<S>(orig + (i * 4 + m) * q.ostride + j * 4, a);
         load_row4<S>(pred + (i * 4 + m) * q.pstride + j * 4, b);
 #pragma unroll
-        for (int t = 0; t < 4; t++) sum = iclip(sum + (a[t] - b[t]), -16384, 16383);
+        for (int t = 0; t < 4; t++) sum = fast ? iclip(sum + (a[t] - b[t]), -16384, 16383) : sum + (a[t] - b[t]);
       }
-      sc.in[i * PI + j] = (int16_t)sum;
+      sc.in[i * PI + j] = (int16_t)sum;  // modulo 2^16
     }
-  } else if (scale == 2) {
+  } else if (scale == 2) {  // 64x64 or 32x32 with `fast`: wraps, and no partial sum leaves the int16 range
     for (int p = tid; p < (size1 * size1) >> 1; p += NT) {  // two outputs (four source columns) per thread and step
       int i = p >> (l1 - 1), j = (p & ((size1 >> 1) - 1)) << 1, s0 = 0, s1 = 0;
       for (int m = 0; m < 2; m++) {
         int a[4], b[4];
         load_row4<S>(orig + (i * 2 + m) * q.ostride + j * 2, a);
         load_row4<S>(pred + (i * 2 + m) * q.pstride + j * 2, b);
-        s0 = iclip(s0 + (a[0] - b[0]), -16384, 16383); s0 = iclip(s0 + (a[1] - b[1]), -16384, 16383);
-        s1 = iclip(s1 + (a[2] - b[2]), -16384, 16383); s1 = iclip(s1 + (a[3] - b[3]), -16384, 16383);
+        s0 += (a[0] - b[0]) + (a[1] - b[1]);
+        s1 += (a[2] - b[2]) + (a[3] - b[3]);
       }
       sc.in[i * PI + j] = (int16_t)s0;
       sc.in[i * PI + j + 1] = (int16_t)s1;
     }
-  } else {
+  } else {  // 128x128 with `fast`: saturates
     for (int p = tid; p < size1 * size1; p += NT) {
       int i = p >> l1, j = p & (size1 - 1), sum = 0;
       for (int m = 0; m < scale; m++)
