@@ -93,6 +93,66 @@ def rand_plane(rng, h, w, bitdepth, hbd, smooth=False):
     return a
 
 
+ME_EXT = 160 - 16  # clip_mv: a vector takes a block at most PADDING_Y - 16 samples outside the picture (common/inter_prediction.c:51-63)
+
+
+def edge_search(rng, padded, fw, fh, size, width, height, sign, bitdepth):
+    """A motion search at the picture's edges, for the block searches of `size` (clip_mv's block) predicting width x height.
+    Returns (xpos, ypos, org, mvc, mvp, near): the block sits in the first or last block row or column or a corner, and org (size x size)
+    copies the padded reference (a 2-D array with a 160-sample border) at a displacement beyond or just inside clip_mv's limit on one or both
+    axes (+-0..20 samples), wholly right of or below the picture (split_mv's pic_w - xpos / pic_h - ypos clamp), or, for left-column blocks,
+    more than `height` rows up (split_mv's -xpos - height bound).  The content there is border-replicated, so it is also found past the
+    limit: the cost minimum lies where clip_mv does not let the search go.  mvc and mvp are quarter-pel vectors with `sign` applied; mvp
+    either sits at the target or thousands of quarter-pels away (the long mv_len codes).  near(n) draws n whole-sample candidates around it."""
+    lastx, lasty = (fw - size) // size * size, (fh - size) // size * size
+    kind = int(rng.integers(0, 4))
+    if kind == 3:  # left column, vertical vector beyond -height
+        xpos, ypos = 0, int(rng.integers(0, fh // size)) * size
+    else:
+        while True:
+            xpos = [0, lastx, int(rng.integers(0, fw // size)) * size][int(rng.integers(0, 3))]
+            ypos = [0, lasty, int(rng.integers(0, fh // size)) * size][int(rng.integers(0, 3))]
+            if xpos in (0, lastx) or ypos in (0, lasty):
+                break
+
+    def at_limit(pos, f):
+        k = int(rng.integers(0, 21)) * int(rng.choice([-1, 1]))
+        return (-ME_EXT - pos - k) if rng.integers(0, 2) else (f + ME_EXT - size - pos + k)
+
+    def outside(pos, f, b):  # wholly past the far edge or more than b samples before the near one, within clip_mv's reach
+        return int(rng.integers(f - pos + 1, f + ME_EXT - size - pos + 1)) if rng.integers(0, 2) else int(rng.integers(-ME_EXT - pos, -pos - b))
+
+    free = lambda: int(rng.integers(-6, 7))
+    if kind == 0:
+        tx, ty = [(at_limit(xpos, fw), free()), (free(), at_limit(ypos, fh)), (at_limit(xpos, fw), at_limit(ypos, fh))][int(rng.integers(0, 3))]
+    elif kind == 1:
+        tx, ty = [(outside(xpos, fw, width), free()), (free(), outside(ypos, fh, height)), (outside(xpos, fw, width), at_limit(ypos, fh))][int(rng.integers(0, 3))]
+    elif kind == 2:
+        tx, ty = at_limit(xpos, fw), outside(ypos, fh, height)
+    else:
+        tx, ty = free(), -height - int(rng.integers(1, 48))
+    # the border replicates the edge samples, so a source clamped into the 160-sample border holds the same block
+    sy, sx = min(max(ypos + ty, -160), fh + 160 - size), min(max(xpos + tx, -160), fw + 160 - size)
+    org = np.clip(padded[160 + sy:160 + sy + size, 160 + sx:160 + sx + size].astype(int) + rng.integers(-2, 3, (size, size)), 0, (1 << bitdepth) - 1)
+    s = -1 if sign else 1
+    mvc = [s * (4 * tx + int(rng.integers(-3, 4))), s * (4 * ty + int(rng.integers(-3, 4)))]
+    far = lambda: int(rng.integers(-4000, 4001)) if rng.integers(0, 2) else 0
+    mvp = [max(-32768, min(32767, s * 4 * tx + far())), max(-32768, min(32767, s * 4 * ty + far()))]
+    near = lambda n: [[s * (tx + int(rng.integers(-4, 5))), s * (ty + int(rng.integers(-4, 5)))] for _ in range(n)]
+    return xpos, ypos, org, mvc, mvp, near
+
+
+def edge_reach(mvx, mvy, sign, xpos, ypos, fw, fh, size, width, height):
+    """(on a clip limit, through an active split_mv clamp) for a search result: whether the vector lies within the sub-pel stages' reach
+    (3 quarter-pels) of clip_mv's limit on either axis, and whether predicting the block with it clamps the integer offset
+    (common/inter_prediction.c:121-131, lower bounds on xpos for both axes as in the reference)"""
+    x, y = (-mvx, -mvy) if sign else (mvx, mvy)
+    lims = ((xpos, x, -ME_EXT), (xpos, x, fw + ME_EXT - size), (ypos, y, -ME_EXT), (ypos, y, fh + ME_EXT - size))
+    on_limit = any(abs(4 * (pos - lim) + v) <= 3 for pos, v, lim in lims)
+    hi, vi = x >> 2, y >> 2
+    return on_limit, hi > fw - xpos or hi < -xpos - width or vi > fh - ypos or vi < -xpos - height
+
+
 def full_scale_planes(h, w, maxv):
     """reconstructions whose intra neighbours sit at 0 and 2^bd-1: uniform, and stripes that put one of the top row and left column at 2^bd-1 and
     alternate the other (the planar pre-filter's int16 input reaches 8 (2^bd-1), 32760 at 12 bits)"""

@@ -4,7 +4,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from _libs import oracle, ref, aligned, P, sdt, sfx, rand_plane, full_scale_planes
+from _libs import oracle, ref, aligned, P, sdt, sfx, rand_plane, full_scale_planes, edge_search, edge_reach
 from _refstructs import Frame as HFrame, random_blkinfo
 
 pytestmark = pytest.mark.gpu
@@ -316,59 +316,107 @@ def test_batch_sad(tb, hbd, bd):
                 assert got64[i] == getattr(O, "orc_ssd_" + s)(a, b, cur.sy, href.sy, bw, bh), i
 
 
-def build_me_items(tb, rng, n, w, h, cur, href, dcur, dref, esz, sizes=(8, 16, 32, 64), speed=0):
+def me_form(bw, bh, speed, esz):
+    """the search form a batch gives an item, restated from MeClassOf / me_class (tb_kernels.cuh): the whole CTA for speed 0 and >= 2048
+    samples in a multiple of 32 rows, four per warp for 8-bit speed-0 blocks of <= 64 samples in multiples of 4, one warp otherwise"""
+    if speed == 0 and bw * bh >= 2048 and bh % 32 == 0:
+        return "team"
+    if esz == 1 and speed == 0 and bw * bh <= 64 and not (bw | bh) & 3:
+        return "quad"
+    return "warp"
+
+
+def me_batch(tb, rng, hbd, bd, w, h, n, edge, sizes, speed, bip):
+    """n searches on a w x h frame pair in one tb_motion_estimate_batch, the last `edge` of them placed at the picture's edges (edge_search,
+    signs alternating; their blocks come from a buffer of their own), each against the oracle.  Returns (differences, reach, forms):
+    reach[sign] counts the edge results on a clip_mv limit / through an active split_mv clamp (edge_reach), forms the search forms the edge
+    items were given."""
+    s = sfx(hbd)
+    esz = 2 if hbd else 1
+    href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
     rptr, rst = dref.plane(0); optr, ost = dcur.plane(0)
+    dorg = tb.DevBuf(max(edge, 1) * 128 * 128 * esz)
     items = np.zeros(n, tb.ME_ITEM)
-    cands = []
-    meta = []
+    orgs = np.zeros((max(edge, 1), 128 * 128), sdt(hbd))
+    cands, meta = [], []
     for i in range(n):
+        e = i - (n - edge)
         size = int(rng.choice(sizes))
         part = int(rng.integers(0, 4))
         bw, bh, ox, oy = size, size, 0, 0
         if part == 1: bh = size // 2; oy = int(rng.integers(0, 2)) * bh
         if part == 2: bw = size // 2; ox = int(rng.integers(0, 2)) * bw
         if part == 3: bw = bh = size // 2; ox = int(rng.integers(0, 2)) * bw; oy = int(rng.integers(0, 2)) * bh
-        xpos = int(rng.integers(0, w // size)) * size; ypos = int(rng.integers(0, h // size)) * size
-        sign = int(rng.integers(0, 2))
         nc = int(rng.integers(0, 9))
         if speed != 0 and nc == 0:
             nc = 1
-        cc = rng.integers(-12, 12, (nc, 2)).astype(np.int16)
-        mvc = rng.integers(-40, 40, 2); mvp = rng.integers(-40, 40, 2)
         lam = float(rng.uniform(2.0, 60.0))
-        items[i] = (optr + ((ypos + oy) * ost + xpos + ox) * esz, rptr + ((ypos + oy) * rst + xpos + ox) * esz, ost, rst, xpos, ypos, size, bw, bh, sign,
+        if e < 0:
+            xpos = int(rng.integers(0, w // size)) * size; ypos = int(rng.integers(0, h // size)) * size
+            sign = int(rng.integers(0, 2))
+            cc = rng.integers(-12, 12, (nc, 2)).astype(np.int16)
+            mvc = rng.integers(-40, 40, 2); mvp = rng.integers(-40, 40, 2)
+            org = cur.y[ypos:ypos + size, xpos:xpos + size]
+            po, so = optr + ((ypos + oy) * ost + xpos + ox) * esz, ost
+        else:
+            sign = e % 2
+            xpos, ypos, org, mvc, mvp, near = edge_search(rng, href.Y, w, h, size, bw, bh, sign, bd)
+            cc = np.array(near(nc), np.int16).reshape(nc, 2)
+            orgs[e, :size * size] = org.reshape(-1)
+            po, so = dorg.ptr + (e * 128 * 128 + oy * size + ox) * esz, size
+        items[i] = (po, rptr + ((ypos + oy) * rst + xpos + ox) * esz, so, rst, xpos, ypos, size, bw, bh, sign,
                     mvc[0], mvc[1], mvp[0], mvp[1], sum(len(c) for c in cands), nc, lam)
         cands.append(cc)
-        meta.append((size, bw, bh, ox, oy, xpos, ypos, sign, cc, mvc, mvp, lam))
+        meta.append((np.array(org), e >= 0, size, bw, bh, ox, oy, xpos, ypos, sign, cc, mvc, mvp, lam))
+    dorg.upload(orgs)
     call = np.concatenate(cands + [np.zeros((1, 2), np.int16)]).astype(np.int16)
-    return items, call, meta
-
-
-@pytest.mark.parametrize("hbd,bd", BD)
-@pytest.mark.parametrize("speed,bip", [(0, 1), (0, 0), (1, 0), (2, 0), (1, 1)])
-def test_batch_motion_estimate(tb, hbd, bd, speed, bip):
-    rng = np.random.default_rng(108 + speed * 7 + bip)
-    s = sfx(hbd)
-    w, h = 256, 192
-    esz = 2 if hbd else 1
-    href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
-    n = 160
-    items, call, meta = build_me_items(tb, rng, n, w, h, cur, href, dcur, dref, esz, speed=speed)
     d_items = tb.DevBuf.from_array(items); d_c = tb.DevBuf.from_array(call); d_out = tb.DevBuf(8 * n)
     tb.check(tb.lib.tb_motion_estimate_batch(d_items.ptr, n, d_c.ptr, esz, bd, speed, bip, w, h, d_out.ptr))
     got = d_out.download(tb.ME_RESULT, n)
-    bad = []
-    for i, (size, bw, bh, ox, oy, xpos, ypos, sign, cc, mvc, mvp, lam) in enumerate(meta):
+    bad, reach, forms = [], np.zeros((2, 2), int), {True: set(), False: set()}
+    for i, (blk, is_edge, size, bw, bh, ox, oy, xpos, ypos, sign, cc, mvc, mvp, lam) in enumerate(meta):
         org = aligned((size, size), sdt(hbd))
-        org[...] = cur.y[ypos:ypos + size, xpos:xpos + size]
+        org[...] = blk
         m0 = (C.c_int16 * 2)(0, 0)
         cands = (C.c_int16 * (2 * max(len(cc), 1)))(*[int(v) for v in cc.reshape(-1)] or [0, 0])
         cost = getattr(O, "orc_motion_estimate_" + s)(P(org, oy * size + ox), P(href.Y, href.origin(0) + (ypos + oy) * href.sy + xpos + ox), size, href.sy, bw, bh, m0,
                                                        (C.c_int16 * 2)(int(mvc[0]), int(mvc[1])), (C.c_int16 * 2)(int(mvp[0]), int(mvp[1])), C.c_double(lam), speed, bd,
                                                        sign, w, h, xpos, ypos, cands, len(cc), bip)
-        if (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"])) != (cost & 0xffffffff, m0[0], m0[1]):
-            bad.append((i, size, bw, bh, sign, (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"])), (cost, m0[0], m0[1])))
-    assert not bad, bad[:8]
+        res = (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"]))
+        if res != (cost & 0xffffffff, m0[0], m0[1]):
+            bad.append((w, h, i, is_edge, size, bw, bh, xpos, ypos, sign, len(cc), res, (cost, m0[0], m0[1])))
+        forms[is_edge].add(me_form(bw, bh, speed, esz))
+        if is_edge:
+            reach[sign] += edge_reach(res[1], res[2], sign, xpos, ypos, w, h, size, bw, bh)
+    assert not edge or forms[True] == forms[False], forms  # every search form the batch uses gets edge items
+    return bad, reach, forms[True]
+
+
+def me_batches(tb, hbd, bd, seed, dims, n, edge, sizes, speed, bip):
+    """me_batch on each frame size of dims; the differences, reach and forms of all of them"""
+    rng = np.random.default_rng(seed)
+    bad, reach, forms = [], np.zeros((2, 2), int), set()
+    for w, h in dims:
+        b, r, f = me_batch(tb, rng, hbd, bd, w, h, n, edge, sizes, speed, bip)
+        bad += b; reach += r; forms |= f
+    return bad, reach, forms
+
+
+# the edge searches' results per sign on a clip_mv limit / through an active split_mv clamp, at least, as fractions of the edge items of one
+# sign (the oracle's results for the same seeded items reach 0.22..0.39 / 0.89..0.98, and 0.47..0.53 / 0.75..0.87 in the bi-directional search)
+ME_EDGE_REACH = np.array([0.15, 0.75])
+ME_BI_EDGE_REACH = np.array([0.3, 0.55])
+EDGE_DIMS = ((256, 192), (200, 136))
+
+
+@pytest.mark.parametrize("hbd,bd", BD)
+@pytest.mark.parametrize("speed,bip", [(0, 1), (0, 0), (1, 0), (2, 0), (1, 1)])
+def test_batch_motion_estimate(tb, hbd, bd, speed, bip):
+    """every search form (one warp, four per warp, the CTA team) at random positions and at the picture's edges"""
+    bad, reach, forms = me_batches(tb, hbd, bd, 108 + speed * 7 + bip, EDGE_DIMS, 160, 64, (8, 16, 32, 64), speed, bip)
+    assert not bad, (len(bad), bad[:8])
+    assert forms == ({"warp", "team", "quad"} if speed == 0 and not hbd else {"warp", "team"} if speed == 0 else {"warp"}), forms
+    assert (reach >= ME_EDGE_REACH * 64).all(), reach
 
 
 @pytest.mark.parametrize("hbd,bd", BD)
@@ -376,51 +424,19 @@ def test_batch_motion_estimate(tb, hbd, bd, speed, bip):
 def test_motion_estimate_small_blocks(tb, hbd, bd, sizes, n, bip):
     """blocks of <= 64 samples: four searches share a warp on 8-bit frames (quad_motion_estimate), incl. the wide-SAD candidates of
     8x8 partitions of 16x16 coding blocks; same results as the oracle"""
-    rng = np.random.default_rng(137 + n)
-    s = sfx(hbd)
-    w, h = 256, 192
-    esz = 2 if hbd else 1
-    href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
-    items, call, meta = build_me_items(tb, rng, n, w, h, cur, href, dcur, dref, esz, sizes=sizes, speed=0)
-    d_items = tb.DevBuf.from_array(items); d_c = tb.DevBuf.from_array(call); d_out = tb.DevBuf(8 * n)
-    tb.check(tb.lib.tb_motion_estimate_batch(d_items.ptr, n, d_c.ptr, esz, bd, 0, bip, w, h, d_out.ptr))
-    got = d_out.download(tb.ME_RESULT, n)
-    bad = []
-    for i, (size, bw, bh, ox, oy, xpos, ypos, sign, cc, mvc, mvp, lam) in enumerate(meta):
-        org = aligned((size, size), sdt(hbd))
-        org[...] = cur.y[ypos:ypos + size, xpos:xpos + size]
-        m0 = (C.c_int16 * 2)(0, 0)
-        cands = (C.c_int16 * (2 * max(len(cc), 1)))(*[int(v) for v in cc.reshape(-1)] or [0, 0])
-        cost = getattr(O, "orc_motion_estimate_" + s)(P(org, oy * size + ox), P(href.Y, href.origin(0) + (ypos + oy) * href.sy + xpos + ox), size, href.sy, bw, bh, m0,
-                                                       (C.c_int16 * 2)(int(mvc[0]), int(mvc[1])), (C.c_int16 * 2)(int(mvp[0]), int(mvp[1])), C.c_double(lam), 0, bd,
-                                                       sign, w, h, xpos, ypos, cands, len(cc), bip)
-        if (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"])) != (cost & 0xffffffff, m0[0], m0[1]):
-            bad.append((i, size, bw, bh, sign, len(cc), (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"])), (cost, m0[0], m0[1])))
+    bad, reach, forms = me_batches(tb, hbd, bd, 137 + n, EDGE_DIMS, n, n // 2, sizes, 0, bip)
     assert not bad, (len(bad), bad[:6])
+    assert ("quad" in forms) == (not hbd), forms
+    assert (reach >= ME_EDGE_REACH * (n // 2)).all(), reach
 
 
 @pytest.mark.parametrize("hbd,bd", BD)
 def test_motion_estimate_large_blocks(tb, hbd, bd):
     """64x64 .. 128x128 prediction blocks are searched by a whole CTA (four warps on row bands); same results as the oracle"""
-    rng = np.random.default_rng(131)
-    s = sfx(hbd)
-    w, h = 384, 256
-    esz = 2 if hbd else 1
-    href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
-    n = 36
-    items, call, meta = build_me_items(tb, rng, n, w, h, cur, href, dcur, dref, esz, sizes=(64, 128), speed=0)
-    d_items = tb.DevBuf.from_array(items); d_c = tb.DevBuf.from_array(call); d_out = tb.DevBuf(8 * n)
-    tb.check(tb.lib.tb_motion_estimate_batch(d_items.ptr, n, d_c.ptr, esz, bd, 0, 1, w, h, d_out.ptr))
-    got = d_out.download(tb.ME_RESULT, n)
-    for i, (size, bw, bh, ox, oy, xpos, ypos, sign, cc, mvc, mvp, lam) in enumerate(meta):
-        org = aligned((size, size), sdt(hbd))
-        org[...] = cur.y[ypos:ypos + size, xpos:xpos + size]
-        m0 = (C.c_int16 * 2)(0, 0)
-        cands = (C.c_int16 * (2 * max(len(cc), 1)))(*[int(v) for v in cc.reshape(-1)] or [0, 0])
-        cost = getattr(O, "orc_motion_estimate_" + s)(P(org, oy * size + ox), P(href.Y, href.origin(0) + (ypos + oy) * href.sy + xpos + ox), size, href.sy, bw, bh, m0,
-                                                       (C.c_int16 * 2)(int(mvc[0]), int(mvc[1])), (C.c_int16 * 2)(int(mvp[0]), int(mvp[1])), C.c_double(lam), 0, bd,
-                                                       sign, w, h, xpos, ypos, cands, len(cc), 1)
-        assert (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"])) == (cost & 0xffffffff, m0[0], m0[1]), (i, size, bw, bh)
+    bad, reach, forms = me_batches(tb, hbd, bd, 131, ((384, 256), (200, 136)), 36, 18, (64, 128), 0, 1)
+    assert not bad, (len(bad), bad[:6])
+    assert forms == {"warp", "team"}, forms
+    assert (reach >= ME_EDGE_REACH * 18).all(), reach
 
 
 @pytest.mark.parametrize("hbd,bd", BD)
@@ -430,13 +446,16 @@ def test_batch_interp(tb, hbd, bd):
     w, h = 256, 192
     esz = 2 if hbd else 1
     href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
-    n = 400
+    # the last `edge` items sit at the picture's edges with vectors at or past clip_mv's limit (edge_search), then clipped; 128-wide and
+    # 128-tall luma blocks go through warp_interp_strips_u8 on 8-bit frames, as in the RD loop
+    n, edge = 600, 200
     items = np.zeros(n, tb.INTERP_ITEM)
-    out = tb.DevBuf(n * 64 * 64 * esz)
+    out = tb.DevBuf(n * 128 * 128 * esz)
     meta = []
+    clamped = 0
     for i in range(n):
         chroma = int(i % 3 == 2)
-        size = int(rng.choice([4, 8, 16, 32, 64] if not chroma else [4, 8, 16, 32]))
+        size = int(rng.choice([4, 8, 16, 32, 64, 128] if not chroma else [4, 8, 16, 32]))
         bw, bh = size, size
         if i % 5 == 1: bw //= 2
         if i % 5 == 2: bh //= 2
@@ -446,15 +465,21 @@ def test_batch_interp(tb, hbd, bd):
         sign = int(rng.integers(0, 2))
         # luma-resolution MV, clipped like the callers do (common/inter_prediction.c:209)
         mv = (C.c_int16 * 2)(int(rng.integers(-600, 600)), int(rng.integers(-600, 600)))
+        if i >= n - edge:
+            lx, ly, _, emv, _, _ = edge_search(rng, href.Y, w, h, size << chroma, bw << chroma, bh << chroma, sign, bd)
+            xpos, ypos = lx >> chroma, ly >> chroma
+            mv[0], mv[1] = emv
         lx, ly = (xpos, ypos) if not chroma else (xpos * 2, ypos * 2)
         O.orc_clip_mv(mv, ly, lx, w, h, bw << chroma, bh << chroma, sign)
+        clamped += i >= n - edge and not chroma and edge_reach(mv[0], mv[1], sign, xpos, ypos, w, h, size, bw, bh)[1]
         ptr, st = dref.plane(1 if chroma else 0)
-        items[i] = (ptr + (ypos * st + xpos) * esz, out.ptr + i * 64 * 64 * esz, st, bw, xpos, ypos, mv[0], mv[1], bw, bh, sign, chroma, pw, ph, 0)
+        items[i] = (ptr + (ypos * st + xpos) * esz, out.ptr + i * 128 * 128 * esz, st, bw, xpos, ypos, mv[0], mv[1], bw, bh, sign, chroma, pw, ph, 0)
         meta.append((chroma, bw, bh, xpos, ypos, sign, mv[0], mv[1], pw, ph))
+    assert clamped >= 100, clamped  # luma edge items predicted through an active split_mv clamp (130 of 133 with this seed)
     d_items = tb.DevBuf.from_array(items)
     for bip in (0, 1):
         tb.check(tb.lib.tb_interp_batch(d_items.ptr, n, esz, bd, bip))
-        got = out.download(sdt(hbd), (n, 64 * 64))
+        got = out.download(sdt(hbd), (n, 128 * 128))
         for i, (chroma, bw, bh, xpos, ypos, sign, mvx, mvy, pw, ph) in enumerate(meta):
             want = aligned((bh, bw), sdt(hbd))
             mv = (C.c_int16 * 2)(mvx, mvy)
@@ -824,37 +849,62 @@ def test_interpolate_frames_1080p(tb):
 
 @pytest.mark.parametrize("hbd,bd", BD)
 def test_batch_motion_estimate_bi_and_combine(tb, hbd, bd):
+    """the bi-directional search at random positions and, for the last 40 items of a batch, at the picture's edges (edge_search; the list
+    entries are quarter-pel vectors, clipped again with the other sign for the second reference); then the element-wise combinations"""
     rng = np.random.default_rng(117)
     s = sfx(hbd)
     esz = 2 if hbd else 1
-    w, h = 192, 128
-    href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
-    href2, _, dref2, _, _ = make_frames(tb, rng, w, h, bd, hbd, shift=(-1, 2))
-    r0, rst = dref.plane(0); r1, _ = dref2.plane(0); optr, ost = dcur.plane(0)
-    n = 60
-    items = np.zeros(n, tb.ME_BI_ITEM)
-    cands = rng.integers(-20, 20, (n, 4, 2)).astype(np.int16)
-    meta = []
-    for i in range(n):
-        size = int(rng.choice([8, 16, 32, 64]))
-        xpos = int(rng.integers(0, w // size)) * size; ypos = int(rng.integers(0, h // size)) * size
-        sign = int(rng.integers(0, 2)); nc = int(rng.integers(0, 5)); lam = float(rng.uniform(2.0, 40.0))
-        mvc = rng.integers(-30, 30, 2); mvp = rng.integers(-30, 30, 2)
-        items[i] = (optr + (ypos * ost + xpos) * esz, r0 + (ypos * rst + xpos) * esz, r1 + (ypos * rst + xpos) * esz, ost, rst, xpos, ypos, size, sign, 0, 0,
-                    mvc[0], mvc[1], mvp[0], mvp[1], 4 * i, nc, lam)
-        meta.append((size, xpos, ypos, sign, nc, lam, mvc, mvp))
-    d_items = tb.DevBuf.from_array(items); d_c = tb.DevBuf.from_array(cands); d_out = tb.DevBuf(8 * n)
-    tb.check(tb.lib.tb_motion_estimate_bi_batch(d_items.ptr, n, d_c.ptr, esz, bd, 1, w, h, d_out.ptr))
-    got = d_out.download(tb.ME_RESULT, n)
-    for i, (size, xpos, ypos, sign, nc, lam, mvc, mvp) in enumerate(meta):
-        org = aligned((size, size), sdt(hbd))
-        org[...] = cur.y[ypos:ypos + size, xpos:xpos + size]
-        m0 = (C.c_int16 * 2)(0, 0)
-        cc = (C.c_int16 * 8)(*[int(v) for v in cands[i].reshape(-1)])
-        cost = getattr(O, "orc_motion_estimate_bi_" + s)(P(org), P(href.Y, href.origin(0) + ypos * href.sy + xpos), P(href2.Y, href2.origin(0) + ypos * href2.sy + xpos), size,
-                                                          href.sy, size, size, m0, (C.c_int16 * 2)(int(mvc[0]), int(mvc[1])), (C.c_int16 * 2)(int(mvp[0]), int(mvp[1])),
-                                                          C.c_double(lam), bd, sign, w, h, xpos, ypos, cc, nc, 1)
-        assert (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"])) == (cost, m0[0], m0[1]), (i, size, sign, nc)
+    n, edge = 100, 40
+    reach = np.zeros((2, 2), int)
+    for w, h in ((192, 128),) + EDGE_DIMS:
+        href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
+        href2, _, dref2, _, _ = make_frames(tb, rng, w, h, bd, hbd, shift=(-1, 2))
+        r0, rst = dref.plane(0); r1, _ = dref2.plane(0); optr, ost = dcur.plane(0)
+        items = np.zeros(n, tb.ME_BI_ITEM)
+        cands = rng.integers(-20, 20, (n, 4, 2)).astype(np.int16)
+        dorg = tb.DevBuf(edge * 64 * 64 * esz)
+        orgs = np.zeros((edge, 64 * 64), sdt(hbd))
+        meta = []
+        for i in range(n):
+            size = int(rng.choice([8, 16, 32, 64]))
+            nc = int(rng.integers(0, 5)); lam = float(rng.uniform(2.0, 40.0))
+            e = i - (n - edge)
+            if e < 0:
+                xpos = int(rng.integers(0, w // size)) * size; ypos = int(rng.integers(0, h // size)) * size
+                sign = int(rng.integers(0, 2))
+                mvc = rng.integers(-30, 30, 2); mvp = rng.integers(-30, 30, 2)
+                org = cur.y[ypos:ypos + size, xpos:xpos + size]
+                po, so = optr + (ypos * ost + xpos) * esz, ost
+            else:
+                sign = e % 2
+                xpos, ypos, org, mvc, mvp, near = edge_search(rng, href.Y, w, h, size, size, size, sign, bd)
+                cands[i] = [[4 * v + int(rng.integers(-3, 4)) for v in c] for c in near(4)]
+                orgs[e, :size * size] = org.reshape(-1)
+                po, so = dorg.ptr + e * 64 * 64 * esz, size
+            items[i] = (po, r0 + (ypos * rst + xpos) * esz, r1 + (ypos * rst + xpos) * esz, so, rst, xpos, ypos, size, sign, 0, 0,
+                        mvc[0], mvc[1], mvp[0], mvp[1], 4 * i, nc, lam)
+            meta.append((np.array(org), e >= 0, size, xpos, ypos, sign, nc, lam, mvc, mvp))
+        dorg.upload(orgs)
+        d_items = tb.DevBuf.from_array(items); d_c = tb.DevBuf.from_array(cands); d_out = tb.DevBuf(8 * n)
+        tb.check(tb.lib.tb_motion_estimate_bi_batch(d_items.ptr, n, d_c.ptr, esz, bd, 1, w, h, d_out.ptr))
+        got = d_out.download(tb.ME_RESULT, n)
+        for i, (blk, is_edge, size, xpos, ypos, sign, nc, lam, mvc, mvp) in enumerate(meta):
+            org = aligned((size, size), sdt(hbd))
+            org[...] = blk
+            m0 = (C.c_int16 * 2)(0, 0)
+            cc = (C.c_int16 * 8)(*[int(v) for v in cands[i].reshape(-1)])
+            cost = getattr(O, "orc_motion_estimate_bi_" + s)(P(org), P(href.Y, href.origin(0) + ypos * href.sy + xpos), P(href2.Y, href2.origin(0) + ypos * href2.sy + xpos), size,
+                                                              href.sy, size, size, m0, (C.c_int16 * 2)(int(mvc[0]), int(mvc[1])), (C.c_int16 * 2)(int(mvp[0]), int(mvp[1])),
+                                                              C.c_double(lam), bd, sign, w, h, xpos, ypos, cc, nc, 1)
+            res = (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"]))
+            assert res == (cost, m0[0], m0[1]), (w, h, i, is_edge, size, xpos, ypos, sign, nc)
+            if is_edge:
+                reach[sign] += np.logical_or(*[edge_reach(res[1], res[2], sg, xpos, ypos, w, h, size, size, size) for sg in (sign, 1 - sign)])
+        if (w, h) == (192, 128):
+            first = w, h, href, cur, dref, dcur
+    assert (reach >= ME_BI_EDGE_REACH * 3 * edge // 2).all(), reach
+    w, h, href, cur, dref, dcur = first
+    r0, rst = dref.plane(0); optr, ost = dcur.plane(0)
     # element-wise combinations on resident frames
     m = 90
     citems = np.zeros(m, tb.COMBINE_ITEM)

@@ -3,13 +3,17 @@ built from /root/reference by oracle/Makefile).  CPU only.  Skipped when oracle/
 import ctypes as C
 import numpy as np
 import pytest
-from _libs import oracle, ref, ref_enc, aligned, P, sdt, sfx, rand_plane, full_scale_planes
+from _libs import oracle, ref, ref_enc, aligned, P, sdt, sfx, rand_plane, full_scale_planes, edge_search, edge_reach
 from _refstructs import Frame, random_blkinfo, CdefStrengths, Mv
 
 pytestmark = pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 O = oracle()
 R = ref()
 BD = [(0, 8), (1, 10), (1, 12)]
+# edge trials per sign whose result lies on a clip_mv limit / is predicted through an active split_mv clamp, at least (the seeded trials reach
+# 37..49 / 141..158 of 160 per sign in test_motion_estimate)
+ME_EDGE_REACH = np.array([25, 100])
+ME_BI_EDGE_REACH = np.array([16, 30])  # of 48 per sign: 24..27 / 43..44
 
 
 def test_tables():
@@ -588,6 +592,34 @@ def test_motion_estimate(hbd, bd):
         a = getattr(O, "orc_motion_estimate_" + s)(P(org), refp, size, f.sy, width, height, m0, mvc, mvp, C.c_double(lam), speed, bd, sign, fw, fh, xpos, ypos, cands, nc, bip)
         b = getattr(E, "ref_motion_estimate_" + s)(P(org), refp, size, f.sy, width, height, m1, mvc, mvp, C.c_double(lam), speed, bd, sign, fw, fh, xpos, ypos, cands, nc, bip)
         assert (a, m0[0], m0[1]) == (b, m1[0], m1[1]), (trial, size, width, height, speed, sign, bip)
+    # edge placement: blocks in the first / last row and column whose best match lies at or past clip_mv's limit, on a picture whose width is
+    # a multiple of 16 and on one whose width is not
+    reach = np.zeros((2, 2), int)  # [sign][on a clip limit, through an active split_mv clamp]
+    for fw, fh in ((256, 192), (200, 136)):
+        f = Frame(fw, fh, bd, hbd)
+        f.randomize(rng)
+        getattr(R, "pad_yuv_frame_" + s)(C.byref(f.s))
+        for trial in range(160):
+            size = int(rng.choice([8, 16, 32, 64]))
+            part = trial % 4
+            width, height = (size, size) if part == 0 else ((size, size // 2) if part == 1 else ((size // 2, size) if part == 2 else (size // 2, size // 2)))
+            speed, sign, bip = trial // 4 % 3, trial // 12 % 2, trial // 24 % 2
+            xpos, ypos, blk, mvc, mvp, near = edge_search(rng, f.Y, fw, fh, size, width, height, sign, bd)
+            org = aligned((size, size), sdt(hbd))
+            org[...] = blk
+            nc = int(rng.integers(0 if speed == 0 or (size == 16 and bip) else 1, 7))
+            cl = near(max(nc, 1))
+            cands = (C.c_int16 * (2 * len(cl)))(*[v for c in cl for v in c])
+            lam = float(rng.uniform(2.0, 60.0))
+            m0 = (C.c_int16 * 2)(0, 0); m1 = (C.c_int16 * 2)(0, 0)
+            refp = P(f.Y, f.origin(0) + ypos * f.sy + xpos)
+            args = (size, f.sy, width, height)
+            rest = ((C.c_int16 * 2)(*mvc), (C.c_int16 * 2)(*mvp), C.c_double(lam), speed, bd, sign, fw, fh, xpos, ypos, cands, nc, bip)
+            a = getattr(O, "orc_motion_estimate_" + s)(P(org), refp, *args, m0, *rest)
+            b = getattr(E, "ref_motion_estimate_" + s)(P(org), refp, *args, m1, *rest)
+            assert (a, m0[0], m0[1]) == (b, m1[0], m1[1]), ("edge", fw, trial, xpos, ypos, size, width, height, speed, sign, bip, mvc, mvp, nc)
+            reach[sign] += edge_reach(m0[0], m0[1], sign, xpos, ypos, fw, fh, size, width, height)
+    assert (reach >= ME_EDGE_REACH).all(), reach
 
 
 def _ti_pair(rng, w, h, bd, hbd, hard):
@@ -655,6 +687,31 @@ def test_motion_estimate_bi_and_combine(hbd, bd):
         a = getattr(O, "orc_motion_estimate_bi_" + s)(P(org), p0, p1, size, f0.sy, size, size, m0, mvc, mvp, C.c_double(lam), bd, sign, fw, fh, xpos, ypos, cands, nc, 1)
         b = getattr(E, "ref_motion_estimate_bi_" + s)(P(org), p0, p1, size, f0.sy, size, size, m1, mvc, mvp, C.c_double(lam), bd, sign, fw, fh, xpos, ypos, cands, nc, 1)
         assert (a, m0[0], m0[1]) == (b, m1[0], m1[1]), (trial, size, sign, nc)
+    # edge placement (see test_motion_estimate); the list entries are quarter-pel vectors, and a vector clipped for one reference is clipped
+    # again with the other sign for the second
+    reach = np.zeros((2, 2), int)
+    for fw, fh in ((256, 192), (200, 136)):
+        f0 = Frame(fw, fh, bd, hbd); f0.randomize(rng)
+        f1 = Frame(fw, fh, bd, hbd)
+        f1.y[...] = np.clip(np.roll(f0.y.astype(int), (2, 3), axis=(0, 1)) + rng.integers(-4, 5, f0.y.shape), 0, (1 << bd) - 1)
+        for f in (f0, f1):
+            getattr(R, "pad_yuv_frame_" + s)(C.byref(f.s))
+        for trial in range(48):
+            size = [8, 16, 32, 64][trial % 4]; sign = trial // 4 % 2
+            xpos, ypos, blk, mvc, mvp, near = edge_search(rng, f0.Y, fw, fh, size, size, size, sign, bd)
+            org = aligned((size, size), sdt(hbd))
+            org[...] = blk
+            nc = int(rng.integers(0, 5))
+            cands = (C.c_int16 * 8)(*[4 * v + int(rng.integers(-3, 4)) for c in near(4) for v in c])
+            lam = float(rng.uniform(2.0, 40.0))
+            m0 = (C.c_int16 * 2)(0, 0); m1 = (C.c_int16 * 2)(0, 0)
+            p0 = P(f0.Y, f0.origin(0) + ypos * f0.sy + xpos); p1 = P(f1.Y, f1.origin(0) + ypos * f1.sy + xpos)
+            rest = ((C.c_int16 * 2)(*mvc), (C.c_int16 * 2)(*mvp), C.c_double(lam), bd, sign, fw, fh, xpos, ypos, cands, nc, 1)
+            a = getattr(O, "orc_motion_estimate_bi_" + s)(P(org), p0, p1, size, f0.sy, size, size, m0, *rest)
+            b = getattr(E, "ref_motion_estimate_bi_" + s)(P(org), p0, p1, size, f0.sy, size, size, m1, *rest)
+            assert (a, m0[0], m0[1]) == (b, m1[0], m1[1]), ("edge", fw, trial, xpos, ypos, size, sign, mvc, mvp, nc)
+            reach[sign] += np.logical_or(*[edge_reach(m0[0], m0[1], sg, xpos, ypos, fw, fh, size, size, size) for sg in (sign, 1 - sign)])
+    assert (reach >= ME_BI_EDGE_REACH).all(), reach
     # element-wise combinations: op 0 against average_blocks_all, op 2 against block_avg_simd, op 1 against its definition
     from _refstructs import Mv
     class BlockPos(C.Structure):

@@ -2,7 +2,7 @@
 
 One table of cases (CASES) drives every test here:
   CPU  oracle/_ref/Thorenc_rdocheck with TB_RDO_VERIFY=1: every super block of every case, decided by thor_b200/csrc/tb_rdo.h over the plain-C
-       oracle and by the reference's process_block() on the same encoder state, must be identical; four cases also run with eight simulated warps.
+       oracle and by the reference's process_block() on the same encoder state, must be identical; five cases also run with eight simulated warps.
   GPU  every case captured with the reference (oracle/_ref/Thorenc_capture); all 8-bit frames of all cases decided in ONE tb_rdo_encode_frames()
        launch, all 10-bit frames in a second one, all 12-bit frames in a third.  Frames of one launch differ in size, qp, speed and options.  Every
        frame must return the reference's reconstruction, block state and cost per super block, and the leaf lists and coefficients that
@@ -11,7 +11,11 @@ One table of cases (CASES) drives every test here:
 The cases reach what qp 32 on smooth content does not: large coefficients and saturation in the transform chain (low qp), frames that are nearly
 all skipped (qp 51), samples at 0 and 2^bd-1 in prediction, bipred average and reconstruction, intra blocks in inter frames (a scene cut), local
 motion, cfl_inter, encoder speeds 1 and 3, block contexts off, no tb split, intra_rdo 0, no early skip, two references, and 12 bits, where the box
-sum of a 128x128 transform can wrap in int16 (hdb_q51_12 codes an unsplit 128x128 block in every frame)."""
+sum of a 128x128 transform can wrap in int16 (hdb_q51_12 codes an unsplit 128x128 block in every frame).  The two fast pans hold vectors of 80
+samples and more, the first of them negative on both axes, and predict thousands of 4x4 cells from wholly outside the picture (split_mv's clamps).
+clip_mv's own limit, 144 samples outside the picture, stays out of the RD loop's reach: a block's search starts from its neighbours' vectors and
+extends them by at most the telescope and hexagon range, and tracked motion does not build up to 144 samples in clips of this length.  The
+motion searches are tested at that limit on their own (test_oracle_vs_ref.py, test_gpu_parity.py)."""
 import ctypes as C
 import os
 import re
@@ -50,7 +54,28 @@ def hard_yuv(path, w, h, n, bitdepth=8, seed=11):
                 f.write(p.astype(np.uint8 if bitdepth == 8 else "<u2").tobytes())
 
 
-CONTENT = {"synth": synth_yuv, "hard": hard_yuv}
+def pan_yuv(path, w, h, n, bitdepth=8, seed=13, pan=(-20, -12)):
+    """Seeded 4:2:0 content panning by `pan` = (x, y) samples per frame: a smooth, aperiodic field (a ramp plus low-pass noise) that holds
+    motion vectors of some 80 samples, negative on both axes for a negative pan, and predicts thousands of 4x4 cells from wholly outside the
+    picture.  (Periodic content aliases: vectors then stop at a fraction of the pan.)"""
+    rng = np.random.default_rng(seed)
+    maxv = (1 << bitdepth) - 1
+    fh, fw = h + abs(pan[1]) * n + 16, w + abs(pan[0]) * n + 16
+    noise = np.fft.ifft2(np.fft.fft2(rng.normal(0, 1, (fh, fw))) * np.exp(-(np.fft.fftfreq(fh)[:, None] ** 2 + np.fft.fftfreq(fw)[None, :] ** 2) * 2000)).real
+    yy, xx = np.mgrid[0:fh, 0:fw]
+    field = 0.25 * xx + 0.15 * yy + noise * (60 / noise.std())
+    field = (field - field.min()) / (field.max() - field.min()) * (maxv - 32) + 16
+    y0, x0 = (abs(pan[1]) * n if pan[1] < 0 else 0), (abs(pan[0]) * n if pan[0] < 0 else 0)
+    with open(path, "wb") as f:
+        for k in range(n):
+            y = field[y0 + pan[1] * k:y0 + pan[1] * k + h, x0 + pan[0] * k:x0 + pan[0] * k + w] + rng.normal(0, 1, (h, w))
+            u = field[y0 + pan[1] * k:y0 + pan[1] * k + h:2, x0 + pan[0] * k:x0 + pan[0] * k + w:2] * 0.5 + maxv / 4
+            v = maxv - u
+            for p in (y, u, v):
+                f.write(np.clip(np.rint(p), 0, maxv).astype(np.uint8 if bitdepth == 8 else "<u2").tobytes())
+
+
+CONTENT = {"synth": synth_yuv, "hard": hard_yuv, "pan_neg": pan_yuv, "pan_pos": lambda path, w, h, n, bitdepth=8: pan_yuv(path, w, h, n, bitdepth, pan=(22, 14))}
 HDB0 = HDB + ["-cdef", "0"]   # tiny frames + CDEF corrupt the reference's header (SURVEY §8c.3)
 CASES = [
     # name               flags                                                         w    h    frames qp bitdepth content
@@ -71,6 +96,10 @@ CASES = [
     ("max_ref2",         HDB0 + ["-max_num_ref", "2"],                                 128, 136, 9, 32, 8,  "synth"),
     ("no_early_skip",    HDB0 + ["-early_skip_thr", "0"],                              128, 136, 9, 32, 8,  "synth"),
     ("ldb_q45_hard",     LDB,                                                          256, 136, 4, 45, 8,  "hard"),
+    # fast pans, (-20, -12) and (+22, +14) samples per frame: the reference's block state holds vectors of up to 80 / 88 samples and predicts
+    # 8916 / 8658 4x4 cells from wholly outside the picture (split_mv's clamps)
+    ("hdb_pan_neg",      HDB0,                                                         384, 256, 9, 32, 8,  "pan_neg"),
+    ("hdb_pan_pos",      HDB0,                                                         384, 256, 9, 32, 8,  "pan_pos"),
     # 12 bits: box sums of 16 residuals leave int16 (128x128 transforms wrap), the inverse transform's second stage can saturate
     ("hdb_q51_12",       HDB0,                                                         128, 136, 5, 51, 12, "synth"),
     ("hdb_q4_hard_12",   HDB0,                                                         128, 136, 5, 4,  12, "hard"),
@@ -114,7 +143,7 @@ def test_every_super_block_matches_reference_process_block(tmp_path, case):
 
 
 @needs_check
-@pytest.mark.parametrize("name", ["cfl_inter_hard", "hdb_q4_hard_10", "hdb_q51_12", "speed1_hard_12"])
+@pytest.mark.parametrize("name", ["cfl_inter_hard", "hdb_q4_hard_10", "hdb_q51_12", "speed1_hard_12", "hdb_pan_neg"])
 def test_overlapped_decision_with_the_device_warp_count(tmp_path, name):
     """the device decides with eight warps per CTA; host threads stand in for them (TBR_HOST_WARPS), see tests/test_rdo_host.py"""
     verify(str(tmp_path), BY_NAME[name], {"TBR_HOST_WARPS": "8"})
