@@ -270,7 +270,7 @@ typedef struct { /* one coded block (a leaf of a super block's quad-tree): every
 #define TB_RDO_SB_COEFFS 24576   /* int16 per super block: quantised coefficients never outnumber the samples (128*128*3/2) */
 typedef struct {
   /* sequence / frame parameters (enc_params, frame_info_t: enc/mainenc.h:35-165) */
-  int32_t width, height, log2_sb_size, bitdepth, sample_bytes;
+  int32_t width, height, log2_sb_size, bitdepth, sample_bytes; /* log2_sb_size 6 or 7, as the reference's encoder allows */
   int32_t frame_type; /* 0 I, 1 P, 2 B (frame_type_t) */
   int32_t qp, num_ref, interp_ref, num_intra_modes;
   double lambda;      /* frame_info.lambda = lambda_coeff * squared_lambda_QP[qp] */

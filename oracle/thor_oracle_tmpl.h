@@ -145,8 +145,18 @@ static const int8_t FN(orc_luma_taps)[2][4][6] = {
 static const int8_t FN(orc_chroma_taps)[8][4] = {{0, 64, 0, 0},  {-2, 58, 10, -2}, {-4, 54, 16, -2}, {-4, 44, 28, -4},
                                                  {-4, 36, 36, -4}, {-4, 28, 44, -4}, {-2, 16, 54, -4}, {-2, 10, 58, -2}};
 
+/* The SIMD edge filters (exactly one fraction non-zero; common/common_kernels_gen.c:1964-1999 luma, :2222-2253 chroma) shift 16-bit
+ * samples right by bitdepth - 10.  At bit depth 8 that count is -2, which the x86 shift takes as a huge unsigned count: every lane becomes
+ * 0 or -1, and the saturating pack makes the prediction 0.  The reference's encoder predicts these zeros (-frame_bitdepth 16 with 8-bit
+ * input); its decoder works in 8-bit samples at bit depth 8 and filters normally, so it does not reconstruct what such an encoder did. */
+static int FN(orc_edge_zero)(int xoff, int yoff, int bitdepth) { return sizeof(S) == 2 && bitdepth == 8 && !xoff != !yoff; }
+
 void FN(orc_interp_luma)(int width, int height, int xoff, int yoff, S *qp, int qstride, const S *ip, int istride, int bipred, int bitdepth) {
   int maxv = (1 << bitdepth) - 1;
+  if (FN(orc_edge_zero)(xoff, yoff, bitdepth)) {
+    for (int i = 0; i < height; i++) memset(qp + i * qstride, 0, (size_t)width * sizeof(S));
+    return;
+  }
   if (xoff == 2 && yoff == 2 && bipred < 2) {
     /* 12-tap 4x4 low-pass at the centre position: corners 0, edges 1, middle 2; (sum+8)>>4 */
     static const int8_t w[4][4] = {{0, 1, 1, 0}, {1, 2, 2, 1}, {1, 2, 2, 1}, {0, 1, 1, 0}};
@@ -178,6 +188,10 @@ void FN(orc_interp_luma)(int width, int height, int xoff, int yoff, S *qp, int q
 /* ---- a8: eighth-pel 4-tap chroma.  common/inter_prediction.c:94-114, common/common_kernels.c:2192-2375 ---- */
 void FN(orc_interp_chroma)(int width, int height, int xoff, int yoff, S *qp, int qstride, const S *ip, int istride, int bitdepth) {
   int maxv = (1 << bitdepth) - 1;
+  if (width > 2 && FN(orc_edge_zero)(xoff, yoff, bitdepth)) { /* 2-wide blocks take the C filter (common/inter_prediction.c:92) */
+    for (int i = 0; i < height; i++) memset(qp + i * qstride, 0, (size_t)width * sizeof(S));
+    return;
+  }
   const int8_t *fh = FN(orc_chroma_taps)[xoff], *fv = FN(orc_chroma_taps)[yoff];
   for (int i = 0; i < height; i++)
     for (int j = 0; j < width; j++) {

@@ -166,3 +166,26 @@ def test_rdo_struct_layouts_match_header(tmp_path):
         dummy = (C.c_uint8 * 64)()
         f.blk = f.leaves = f.leaf_count = f.coeffs = C.addressof(dummy)
         assert t.lib.tb_rdo_encode_frame(C.byref(f)) == t.TB_ERR_CUDA
+
+
+def test_rdo_entry_points_reject_super_block_sizes_the_reference_cannot_produce():
+    """The reference's encoder takes -log2_sb_size 6 or 7 (enc/strings.c:527).  tb_rdo_encode_frames and tb_rdo_batch_upload refuse every other
+    size with TB_ERR_ARG while checking the frame description, before any CUDA call (so this runs with or without a device).  The accepted sizes
+    pass that check and stop at the next one: missing output buffers, and no batch."""
+    import ctypes as C
+    import thor_b200 as t
+    from thor_b200 import rdo_jobs as RJ
+    t.lib.tb_rdo_last_error.restype = C.c_char_p
+    t.lib.tb_rdo_encode_frames.argtypes = [C.c_void_p, C.c_int]
+    t.lib.tb_rdo_batch_upload.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+    dummy = (C.c_uint8 * 64)()
+    for log2_sb in (4, 5, 6, 7, 8):
+        f = RJ.RdoFrame()
+        f.width, f.height, f.log2_sb_size, f.sample_bytes, f.bitdepth, f.qp = 64, 64, log2_sb, 1, 8, 32
+        f.blk = f.leaves = f.leaf_count = f.coeffs = C.addressof(dummy) if log2_sb not in (6, 7) else 0
+        assert t.lib.tb_rdo_encode_frames(C.byref(f), 1) == t.TB_ERR_ARG, log2_sb
+        err = t.lib.tb_rdo_last_error()
+        assert (b"unsupported frame description" in err) == (log2_sb not in (6, 7)) and (b"missing output buffers" in err) == (log2_sb in (6, 7)), (log2_sb, err)
+        assert t.lib.tb_rdo_batch_upload(None, 0, C.byref(f)) == t.TB_ERR_ARG, log2_sb
+        err = t.lib.tb_rdo_last_error()
+        assert (b"unsupported frame description" in err) == (log2_sb not in (6, 7)) and (b"bad slot" in err) == (log2_sb in (6, 7)), (log2_sb, err)

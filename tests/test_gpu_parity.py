@@ -9,7 +9,7 @@ from _refstructs import Frame as HFrame, random_blkinfo
 
 pytestmark = pytest.mark.gpu
 O = oracle()
-BD = [(0, 8), (1, 10), (1, 12)]
+BD = [(0, 8), (1, 8), (1, 10), (1, 12)]  # (1, 8): 8-bit content in 16-bit frames (-frame_bitdepth 16)
 
 
 @pytest.fixture(scope="module")

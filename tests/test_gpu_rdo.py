@@ -47,6 +47,11 @@ CLIPS = {"hdb_10bit_q4_hard": (4, hard_yuv), "hdb_8bit_q51": (51, synth_yuv), "h
     ("hdb_8bit_cfl_inter_hard", HDB + ["-cdef", "0", "-enable_cfl_inter", "1"], 128, 136, 5, (), True),
     ("hdb_8bit_speed1_rect_hard", HDB + ["-cdef", "0", "-encoder_speed", "1"], 200, 72, 5, (), True),
     ("hdb_12bit_q51", HDB + ["-cdef", "0"], 128, 136, 5, ("-bitdepth", "12", "-input_bitdepth", "12"), True),
+    ("hdb_8bit_sb64_rect", HDB + ["-cdef", "0", "-log2_sb_size", "6"], 200, 136, 5, (), True),   # 64x64 super blocks, a partial last column
+    ("hdb_8bit_no_interp", HDB + ["-cdef", "0", "-interp_ref", "0"], 128, 136, 9, (), True),     # B frames without an interpolated reference
+    # 8-bit content in 16-bit frames, where the reference's encoder predicts 0 at one-axis fractions (DESIGN.md §5).  Its decoder filters
+    # these normally, so it does not reconstruct the encoder's frames: encoder outputs only
+    ("hdb_8bit_fb16", HDB + ["-cdef", "0"], 128, 136, 5, ("-frame_bitdepth", "16"), False),
 ])
 def test_device_rd_loop_encode_is_bit_exact(tmp_path, name, flags, w, h, n, extra, decode):
     tmp = str(tmp_path)

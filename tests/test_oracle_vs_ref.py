@@ -9,7 +9,7 @@ from _refstructs import Frame, random_blkinfo, CdefStrengths, Mv
 pytestmark = pytest.mark.skipif(ref() is None, reason="oracle/_ref not built")
 O = oracle()
 R = ref()
-BD = [(0, 8), (1, 10), (1, 12)]
+BD = [(0, 8), (1, 8), (1, 10), (1, 12)]  # (1, 8): 8-bit content in 16-bit frames (-frame_bitdepth 16)
 # edge trials per sign whose result lies on a clip_mv limit / is predicted through an active split_mv clamp, at least (the seeded trials reach
 # 37..49 / 141..158 of 160 per sign in test_motion_estimate)
 ME_EDGE_REACH = np.array([25, 100])

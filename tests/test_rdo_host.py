@@ -26,6 +26,7 @@ CASES = [
     ("ldb_8bit", LDB, 320, 200, 5, ()),
     ("hdb_10bit_B", HDB + ["-cdef", "0"], 128, 136, 9, ("-bitdepth", "10", "-input_bitdepth", "10")),
     ("ldb_10bit", LDB, 256, 200, 4, ("-bitdepth", "10", "-input_bitdepth", "10")),
+    ("hdb_8bit_fb16", HDB + ["-cdef", "0"], 128, 136, 5, ("-frame_bitdepth", "16")),   # 8-bit content in 16-bit frames (DESIGN.md §5)
 ]
 
 
@@ -54,7 +55,7 @@ def test_every_super_block_matches_reference_process_block(tmp_path, name, flags
 
 
 @needs
-@pytest.mark.parametrize("name,flags,w,h,n,extra", CASES[:1] + CASES[2:3])
+@pytest.mark.parametrize("name,flags,w,h,n,extra", CASES[:1] + CASES[2:3] + CASES[5:6])
 def test_whole_encode_through_the_c_abi_is_bit_exact(tmp_path, name, flags, w, h, n, extra):
     tmp = str(tmp_path)
     synth_yuv(os.path.join(tmp, "in.yuv"), w, h, n, 10 if "10bit" in name else 8)

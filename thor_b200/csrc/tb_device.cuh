@@ -317,7 +317,16 @@ __constant__ int8_t c_chroma_taps[8][4] = {{0, 64, 0, 0},  {-2, 58, 10, -2}, {-4
 
 // One luma sample at fractional position (xf,yf) in quarter-pels; ip = integer position.
 // common/inter_prediction.c:146-180.  bip = sequence-level enable_bipred value (0/1/2).
+// Every 16-bit prediction goes through luma_sample / chroma_sample, so they also reproduce the reference's SIMD edge filters
+// (exactly one fraction non-zero, common/common_kernels_gen.c:1964-1999 / :2222-2253) at bit depth 8: these shift 16-bit samples by
+// bitdepth - 10 = -2, which the x86 shift takes as a huge count, and the saturating pack then gives 0.  2-wide chroma blocks take the
+// reference's C filter instead (common/inter_prediction.c:92).  8-bit samples take the _lbd path, which has no such shift: `if constexpr`
+// leaves their code as it was.
+__device__ __forceinline__ bool edge_zero_hbd(int xf, int yf, int maxv) { return maxv == 255 && (xf == 0) != (yf == 0); }
 template <class S> __device__ __forceinline__ int luma_sample(const S *ip, int is, int xf, int yf, int bip, int maxv) {
+  if constexpr (sizeof(S) == 2) {
+    if (edge_zero_hbd(xf, yf, maxv)) return 0;
+  }
   if (xf == 2 && yf == 2 && bip < 2) {
     int s = (int)ip[-is] + ip[-is + 1] + ip[-1] + ip[2] + ip[is - 1] + ip[is + 2] + ip[2 * is] + ip[2 * is + 1] +
             2 * ((int)ip[0] + ip[1] + ip[is] + ip[is + 1]);
@@ -347,8 +356,11 @@ template <class S> __device__ __forceinline__ int luma_sample(const S *ip, int i
   }
   return sat_px((sum + 2048) >> 12, maxv);
 }
-// common/inter_prediction.c:94-114
-template <class S> __device__ __forceinline__ int chroma_sample(const S *ip, int is, int xf, int yf, int maxv) {
+// common/inter_prediction.c:94-114; w = the block's width
+template <class S> __device__ __forceinline__ int chroma_sample(const S *ip, int is, int xf, int yf, int w, int maxv) {
+  if constexpr (sizeof(S) == 2) {
+    if (w > 2 && edge_zero_hbd(xf, yf, maxv)) return 0;
+  }
   const int8_t *fh = c_chroma_taps[xf], *fv = c_chroma_taps[yf];
   int sum = 0;
 #pragma unroll
@@ -399,7 +411,7 @@ __device__ void warp_interp(S *dst, int ds, const S *ref, int rs, int w, int h, 
     const S *q = ip + row * rs + col;
     int v;
     if (xf == 0 && yf == 0) v = q[0];
-    else v = chroma ? chroma_sample<S>(q, rs, xf, yf, maxv) : luma_sample<S>(q, rs, xf, yf, bip, maxv);
+    else v = chroma ? chroma_sample<S>(q, rs, xf, yf, w, maxv) : luma_sample<S>(q, rs, xf, yf, bip, maxv);
     dst[row * ds + col] = (S)v;
   }
 }

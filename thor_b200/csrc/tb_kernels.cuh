@@ -284,7 +284,7 @@ __global__ void interp_frac_kernel(S *dst, int ds, const S *ip, int is, int w, i
   for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < (h << lw); p += gridDim.x * blockDim.x) {
     int row = p >> lw, col = p & (w - 1);
     const S *q = ip + row * is + col;
-    dst[row * ds + col] = (S)(chroma ? chroma_sample<S>(q, is, xf, yf, maxv) : luma_sample<S>(q, is, xf, yf, bip, maxv));
+    dst[row * ds + col] = (S)(chroma ? chroma_sample<S>(q, is, xf, yf, w, maxv) : luma_sample<S>(q, is, xf, yf, bip, maxv));
   }
 }
 template <class S> __global__ void block_avg_kernel(S *p, int sp, const S *r0, int s0, const S *r1, int s1, int w, int h) {

@@ -200,7 +200,7 @@ template <class S> struct DevBackend {
         const S *q = ip + row * rs + col;
         int v;
         if (xf == 0 && yf == 0) v = q[0];
-        else v = chroma ? chroma_sample<S>(q, rs, xf, yf, maxv) : luma_sample<S>(q, rs, xf, yf, bip, maxv);
+        else v = chroma ? chroma_sample<S>(q, rs, xf, yf, w, maxv) : luma_sample<S>(q, rs, xf, yf, bip, maxv);
         dst[row * ds + col] = (S)v;
       }
     }
@@ -797,7 +797,7 @@ template <class S> void fill_ctx(FrameCtx<S> &C, const Slot &D, const tb_rdo_fra
 }
 
 int check_desc(const tb_rdo_frame_t *f) {
-  if (!f || f->num_ref > TB_RDO_MAX_REF || f->num_ref < 0 || f->log2_sb_size > 7 || f->log2_sb_size < 4 || (f->sample_bytes != 1 && f->sample_bytes != 2) || f->width <= 0 ||
+  if (!f || f->num_ref > TB_RDO_MAX_REF || f->num_ref < 0 || (f->log2_sb_size != 6 && f->log2_sb_size != 7) /* the reference's encoder allows 64 and 128 */ || (f->sample_bytes != 1 && f->sample_bytes != 2) || f->width <= 0 ||
       f->height <= 0 || (f->width & 7) || (f->height & 7) || f->interp_ref == 2 || f->qp < 0 || f->qp > 51 ||
       (f->num_ref > 0 && (f->ref_pad < 160 /* clip_mv admits vectors 144 samples outside the frame (+ filter taps): the reference's PADDING_Y */ ||
                           f->ref_stride[0] < f->width + 2 * f->ref_pad))) {
@@ -898,8 +898,8 @@ void tb_rdo_batch_destroy(tb_rdo_batch_t *b) {
 }
 
 int tb_rdo_batch_upload(tb_rdo_batch_t *b, int slot, const tb_rdo_frame_t *f) {
-  if (!b || slot < 0 || slot >= b->nslots) { snprintf(g_err, sizeof(g_err), "tb_rdo_batch_upload: bad slot"); return TB_ERR_ARG; }
   if (check_desc(f) != TB_OK) return TB_ERR_ARG;
+  if (!b || slot < 0 || slot >= b->nslots) { snprintf(g_err, sizeof(g_err), "tb_rdo_batch_upload: bad slot"); return TB_ERR_ARG; }
   if (f->sample_bytes != b->esz) { snprintf(g_err, sizeof(g_err), "tb_rdo_batch_upload: sample size differs from the batch's"); return TB_ERR_ARG; }
   cudaStream_t st = (cudaStream_t)tb_stream();
   Slot &D = b->slots[slot];
