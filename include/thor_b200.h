@@ -308,9 +308,12 @@ int tb_rdo_batch_grid(const tb_rdo_batch_t *b);                                 
  * chain, coefficient bits, SSD/SAD, intra, copies, early skip, idle, total); [11..22] work actually executed (the RD loop is data dependent):
  * searches, integer block SADs, sub-pel probes, search samples (SURVEY 8d: (n_int+1) w h + n_sub ((w+5)(h+5) + w h)), predictions, prediction samples,
  * transform chains, chain samples (3 N^2), intra predictions, intra samples (4N + N^2), SSD/SAD samples (2 w h), super blocks */
-#define TB_RDO_NSTATS 60 /* [23..39]: cycles of searches by coding-block size 8..128 (5), of transform chains by size 4..128 (6), of predictions by size 4..128 (6);
+#define TB_RDO_NSTATS 68 /* [23..39]: cycles of searches by coding-block size 8..128 (5), of transform chains by size 4..128 (6), of predictions by size 4..128 (6);
                             [40..48]: wall cycles of a CTA by decision phase (other, early skip, skip/merge candidates, searches, inter candidates, bipred, intra search,
-                            intra candidates, commit); [49..53]: cycles of the searches of blocks <= 16 by stage (telescope, candidates, hexagon, half-pel, quarter-pel) */
+                            intra candidates, commit); [49..53]: cycles of the searches of blocks <= 16 by stage (telescope, candidates, hexagon, half-pel, quarter-pel);
+                            [54..59]: search phase of an overlapped decision, warp 0 and the last warp {own searches, -, barrier wait}; [60..65]: its bi-prediction
+                            phase, warp 0 {chain, inter candidates, barrier wait} and the last warp {joint search as the helper, inter candidates, barrier wait};
+                            [66..67]: overlapped B-frame decisions whose joint bi-prediction search ran on the helper warp, on warp 0 */
 int tb_rdo_batch_stats(const tb_rdo_batch_t *b, uint64_t *out, int n);
 /* timeline of the last synchronised launch: one entry per super block, in the order they finished.  Times are the GPU's global nanosecond
  * timer (%globaltimer), comparable between SMs.  A super block starts after the super blocks it depends on have ended. */

@@ -40,7 +40,9 @@ enum { PF_INTERP, PF_ME, PF_MEBI, PF_TX, PF_BITS, PF_SSD, PF_INTRA, PF_COPY, PF_
 enum { ST_ME = PF_N, ST_ME_INT, ST_ME_SUB, ST_ME_SAMPLES, ST_IP, ST_IP_SAMPLES, ST_TX, ST_TX_SAMPLES, ST_INTRA, ST_INTRA_SAMPLES, ST_SSD_SAMPLES, ST_SB,
        ST_ME_SZ /* cycles of searches by coding-block size 8..128 */, ST_TX_SZ = ST_ME_SZ + 5 /* chains by transform size 4..128 */, ST_IP_SZ = ST_TX_SZ + 6 /* predictions by width 4..128 */,
        ST_PH = ST_IP_SZ + 6 /* wall cycles of warp 0 by decision phase (tb_rdo.h PH_*) */, ST_MESTAGE = ST_PH + tbr::PH_N /* search stages, coding blocks <= 16 */,
-       ST_X = ST_MESTAGE + 5 /* search phase of a block decision: warp 0 {own searches, -, barrier wait}, warp nw-1 {own searches, -, barrier wait} */, ST_END = ST_X + 6 };
+       ST_X = ST_MESTAGE + 5 /* search phase of a block decision: warp 0 {own searches, -, barrier wait}, warp nw-1 {own searches, -, barrier wait} */,
+       ST_XB = ST_X + 6 /* bi-prediction phase (mark2 6..8): warp 0 {chain, inter candidates, barrier wait}, warp nw-1 {joint search as the helper, inter candidates, barrier wait} */,
+       ST_JOINT = ST_XB + 6 /* overlapped B-frame decisions whose joint bi-prediction search ran {on the helper warp, on warp 0} */, ST_END = ST_JOINT + 2 };
 struct Prof {
   long long *acc;
   int k, k2;
@@ -108,12 +110,15 @@ template <class S> struct DevBackend {
     for (int k = threadIdx.x & 31; k < nwords; k += 32) ((int *)dst)[k] = ((const int *)src)[k];
     __syncwarp();
   }
-  __device__ __forceinline__ void mark2(int k) const {  // per-warp timers of the search phase, kept for warp 0 and the last warp
+  __device__ __forceinline__ void mark2(int k) const {  // per-warp timers of the search phase (k 0..2) and the bi-prediction phase (k 6..8), kept for warp 0 and the last warp
     if ((wid == 0 || wid == nw - 1) && (threadIdx.x & 31) == 0) {
       const long long t = clock64();
       if (k >= 0) sh->prof[ST_X + (wid == 0 ? 0 : 3) + k] += t - sh->t_mark2;
       sh->t_mark2 = t;
     }
+  }
+  __device__ __forceinline__ void count_joint(bool on_helper) const {
+    if (wid == 0 && (threadIdx.x & 31) == 0) sh->prof[ST_JOINT + (on_helper ? 0 : 1)] += 1;
   }
   __device__ __forceinline__ void mark(int k) const {
     if (wid == 0 && (threadIdx.x & 31) == 0) { const long long t = clock64(); sh->prof[ST_PH + k] += t - sh->t_mark; sh->t_mark = t; }
@@ -976,6 +981,9 @@ int tb_rdo_batch_sync(tb_rdo_batch_t *b) {
     }
     fprintf(stderr, "\n[tb_rdo prof] search phase: warp 0 own searches %.0f, barrier wait %.0f | last warp own searches %.0f, barrier wait %.0f  [Mcycles]",
             pr[ST_X] / 1e6, pr[ST_X + 2] / 1e6, pr[ST_X + 3] / 1e6, pr[ST_X + 5] / 1e6);
+    fprintf(stderr, "\n[tb_rdo prof] bi-prediction phase: warp 0 chain %.0f, inter candidates %.0f, barrier wait %.0f | last warp joint search %.0f, inter candidates %.0f, "
+            "barrier wait %.0f  [Mcycles]; joint searches on the helper %llu, on warp 0 %llu",
+            pr[ST_XB] / 1e6, pr[ST_XB + 1] / 1e6, pr[ST_XB + 2] / 1e6, pr[ST_XB + 3] / 1e6, pr[ST_XB + 4] / 1e6, pr[ST_XB + 5] / 1e6, pr[ST_JOINT], pr[ST_JOINT + 1]);
     fprintf(stderr, "\n[tb_rdo prof] search cycles by coding-block size 8..128:");
     for (int k = 0; k < 5; k++) fprintf(stderr, " %.1f%%", 100.0 * (double)pr[ST_ME_SZ + k] / (double)(pr[PF_ME] ? pr[PF_ME] : 1));
     fprintf(stderr, "; transform chains by size 4..128:");

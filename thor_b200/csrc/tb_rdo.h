@@ -22,6 +22,10 @@
 // Not restated (tb_rdo_encode_frame rejects these settings): sync, qmtx, interp_ref == 2, delta QP / rate control, 4:4:4 / 4:0:0.
 #pragma once
 #include <stdint.h>
+#ifndef __CUDACC__
+#include <cstdio>
+#include <cstdlib>
+#endif
 #include "../../include/thor_b200.h"
 
 // TBR_NI: the functions of the control flow exist ONCE in the device code (no inlining at their many call sites): the RD loop is one kernel whose warps run
@@ -114,6 +118,19 @@ TBR_HD inline int downleft_available(int ypos, int xpos, int bw, int bh, int /*f
   return a;
 }
 
+#ifndef __CUDACC__
+// the host build's form of the device's schedule counters (count_joint): printed at exit when TBR_HOST_STATS is set.  The simulated warps never
+// run at the same time, so plain counters suffice
+struct HostCounts {
+  long joint_helper = 0, joint_warp0 = 0;
+  ~HostCounts() {
+    if (getenv("TBR_HOST_STATS"))
+      fprintf(stderr, "[tb_rdo.h] joint bi-prediction searches of overlapped decisions: %ld on the helper warp, %ld on warp 0\n", joint_helper, joint_warp0);
+  }
+};
+inline HostCounts host_counts;
+#endif
+
 // frame-level state the RD loop reads and writes (pointers are in the address space of the build: host or device)
 template <class S> struct FrameCtx {
   int width, height, sb_size, bitdepth, frame_type, qp, qpc, num_ref, interp_ref, num_intra_modes;
@@ -195,6 +212,14 @@ template <class S, class B> struct Rdo {
     const tb_rdo_blk_t b = be.ld_blk(F.blk + index);  // another CTA may have written it: the device backend bypasses L1
     IPred p; p.mv0 = b.mv0; p.mv1 = b.mv1; p.ref_idx0 = b.ref_idx0; p.ref_idx1 = b.ref_idx1; p.bipred_flag = b.bipred_flag;
     return p;
+  }
+  // (diagnostics) an overlapped B-frame decision ran its joint bi-prediction search on the helper warp, or on warp 0 after the chain
+  TBR_HD void count_joint(bool on_helper) {
+#ifdef __CUDACC__
+    be.count_joint(on_helper);
+#else
+    (on_helper ? host_counts.joint_helper : host_counts.joint_warp0)++;
+#endif
   }
   TBR_HD static IPred zero_pred() { IPred p; p.mv0.x = p.mv0.y = p.mv1.x = p.mv1.y = 0; p.ref_idx0 = p.ref_idx1 = 0; p.bipred_flag = 0; return p; }
 
@@ -667,6 +692,12 @@ template <class S, class B> struct Rdo {
     return min_sad;
   }
 
+  // motion_estimate_bi scribbles on the caller's list (:873-881): entries num..3 are zeroed, [4] = mvp (quarter-pel, sic), [5] = 0; the
+  // list length is unchanged, so entries 4 and 5 stay visible to every later search of this super block once the list is that long
+  TBR_HD void scribble_bi(int r0, Mv mvp) {
+    for (int idx = W.mvcand_num[r0]; idx < 4; idx++) { W.mvcand[r0][idx].x = 0; W.mvcand[r0][idx].y = 0; }
+    W.mvcand[r0][4] = mvp; W.mvcand[r0][5].x = 0; W.mvcand[r0][5].y = 0;
+  }
   // search_bipred_prediction_params :1679-1833
   TBR_HD TBR_NI int search_bipred(const BlockInfo &bi, int part, const Mv *mv_center, Mv mvp, int *ref_idx0, int *ref_idx1, Mv *mv_arr0, Mv *mv_arr1, int me_mode) {
     const int size = bi.size;
@@ -676,10 +707,7 @@ template <class S, class B> struct Rdo {
       const S *ref0 = F.ref[r0][0] + bi.ypos * rs + bi.xpos, *ref1 = F.ref[r1][0] + bi.ypos * rs + bi.xpos;
       Mv mv;
       const int sad = be.me_bi(oy, F.org_stride[0], ref0, ref1, rs, size, &mv, mv_center[r0], mvp, F.sqrt_lambda, 0, bi.xpos, bi.ypos, W.mvcand[r0], W.mvcand_num[r0], W.p0_y, W.p1_y);
-      // motion_estimate_bi scribbles on the caller's list (:873-881): entries num..3 are zeroed, [4] = mvp (quarter-pel, sic), [5] = 0; the
-      // list length is unchanged, so entries 4 and 5 stay visible to every later search of this super block once the list is that long
-      for (int idx = W.mvcand_num[r0]; idx < 4; idx++) { W.mvcand[r0][idx].x = 0; W.mvcand[r0][idx].y = 0; }
-      W.mvcand[r0][4] = mvp; W.mvcand[r0][5].x = 0; W.mvcand[r0][5].y = 0;
+      scribble_bi(r0, mvp);
       *ref_idx0 = r0; *ref_idx1 = r1;
       for (int i = 0; i < 4; i++) mv_arr0[i] = mv_arr1[i] = mv;
       return sad;
@@ -770,15 +798,22 @@ template <class S, class B> struct Rdo {
     }
   }
   // the bi-prediction candidates (BIPRED_PART = 0: one partition): search_bipred_prediction_params, a chain of dependent searches, and its tb_param
-  // variants; in B frames at encoder_speed 0 also the candidate of the joint search (me_mode 1)
-  TBR_HD TBR_NI void bipred_cands(BlockInfo &bi, Cand &t, const Mv *mv_center, Mv mvp, bool own, int *pos) {
-    search_bipred(bi, 0, mv_center, mvp, &t.ref_idx0, &t.ref_idx1, t.mv0, t.mv1, 0);
-    t.mode = MODE_BIPRED; t.pb_part = PART_NONE;
-    eval_tbs(bi, t, 0, IDX_BIPRED, own, pos, false);
+  // variants; in B frames at encoder_speed 0 also the candidate of the joint search (me_mode 1).  `joint` splits them between two warps:
+  // JOINT_ELSEWHERE runs the chain and, in place of the joint search, only its scribble on the candidate list; JOINT_ONLY runs the joint search
+  enum { JOINT_HERE = 0, JOINT_ELSEWHERE, JOINT_ONLY };
+  TBR_HD TBR_NI void bipred_cands(BlockInfo &bi, Cand &t, const Mv *mv_center, Mv mvp, bool own, int *pos, int joint) {
+    if (joint != JOINT_ONLY) {
+      search_bipred(bi, 0, mv_center, mvp, &t.ref_idx0, &t.ref_idx1, t.mv0, t.mv1, 0);
+      t.mode = MODE_BIPRED; t.pb_part = PART_NONE;
+      eval_tbs(bi, t, 0, IDX_BIPRED, own, pos, false);
+    }
     if (F.frame_type == B_FRAME && F.speed == 0) {
-      search_bipred(bi, 1, mv_center, mvp, &t.ref_idx0, &t.ref_idx1, t.mv0, t.mv1, 1);
-      t.tb_param = 0;
-      if (own || be.mine(*pos)) eval_cand(bi, t, bi.size, bi.size, IDX_BIPRED + bi.max_tb, false);
+      if (joint == JOINT_ELSEWHERE) scribble_bi(F.interp_ref ? 1 : 0, mvp);
+      else {
+        search_bipred(bi, 1, mv_center, mvp, &t.ref_idx0, &t.ref_idx1, t.mv0, t.mv1, 1);
+        t.mode = MODE_BIPRED; t.pb_part = PART_NONE; t.tb_param = 0;
+        if (own || be.mine(*pos)) eval_cand(bi, t, bi.size, bi.size, IDX_BIPRED + bi.max_tb, false);
+      }
       (*pos)++;
     }
     be.mark(PH_BIPRED);
@@ -791,7 +826,8 @@ template <class S, class B> struct Rdo {
   // Square blocks of inter frames at encoder_speed 0 on more than one warp OVERLAP the sections that do not depend on each other instead:
   //   the references' motion searches run one warp per reference, and nothing else runs beside them;
   //   then warp 0 runs the bi-prediction chain (every search depends on the previous one) and evaluates its candidates, while the others draw the
-  //   inter candidates (one draw = the tb_param variants of one prediction) from a shared counter;
+  //   inter candidates (one draw = the tb_param variants of one prediction) from a shared counter; in B frames the last warp runs the chain's
+  //   joint search first, when the candidate list allows it (see (3));
   //   after a barrier every warp draws the items of the intra-mode search (with intra_rdo, the intra candidates), and the candidate lists the
   //   chain extends are copied to the other warps' replicas.
   // The RD loop is bound by instruction delivery: warps that run different code at the same time slow each other down (searches beside the
@@ -870,7 +906,21 @@ template <class S, class B> struct Rdo {
         be.mark(PH_SEARCH);
         // (3) the RD candidates of the references (overlapped: drawn, while warp 0 runs the bi-prediction chain first)
         const bool do_bipred = F.num_ref > 1 && F.enable_bipred;
-        if (overlap && do_bipred && be.warp() == 0) bipred_cands(bi, t, mv_center, mvp, true, &pos);
+        // The joint bi-prediction search of B frames (motion_estimate_bi, :798-890) reads mv_center[r0], mvp, the source and the references, entries
+        // 0 .. min(num, 4) - 1 of candidate list r0 and whether num < 4, num = the list's length when it runs; it then zeroes entries num..3 and sets
+        // [4] = mvp, [5] = 0 before it reads entries 0..5.  The chain before it (me_mode 0) only appends to list r0 (add_mvcandidate never rewrites an
+        // entry), and every replica of the lists is the same after the replay above.  So when list r0 holds 4 entries or more here, the joint search
+        // reads the same inputs before, beside or after the chain: the last warp (the helper) runs it first on its own replica and evaluates its
+        // candidate, index IDX_BIPRED + max_tb whichever warp evaluates it, then draws inter candidates; warp 0 runs the chain and applies the scribble
+        // (which does not depend on the search's result) where the search stood, and its lists are copied to every replica after the phase.
+        // With a shorter list the chain's appends change what the joint search reads, and warp 0 runs it after the chain as the reference does.
+        const int r0 = F.interp_ref ? 1 : 0;
+        const bool joint = overlap && do_bipred && F.frame_type == B_FRAME, helper = joint && W.mvcand_num[r0] >= 4;
+        if (joint && be.warp() == 0) count_joint(helper);
+        if (overlap) be.mark2(-1);
+        if (overlap && do_bipred && (be.warp() == 0 || (helper && be.warp() == be.nwarps() - 1)))
+          bipred_cands(bi, t, mv_center, mvp, true, &pos, !helper ? JOINT_HERE : be.warp() == 0 ? JOINT_ELSEWHERE : JOINT_ONLY);
+        if (overlap) be.mark2(6);  // (diagnostics) warp 0: the chain; the last warp: the joint search when it is the helper
         const int ntb = bi.max_tb + 1, min_tb = F.speed < 1 ? -1 : 0;  // tb_param -1: no residual (:1990)
         for (int g = overlap ? be.next(0) : 0; g < nrs * bi.max_pb; g = overlap ? be.next(0) : g + 1) {
           const int part = g % bi.max_pb, ref_idx = min_idx + g / bi.max_pb;
@@ -885,7 +935,9 @@ template <class S, class B> struct Rdo {
         }
         be.mark(PH_INTER_CAND);
         if (overlap) {  // the intra-mode search, once the chain and the inter candidates are done
+          be.mark2(7);
           be.cta_sync();
+          be.mark2(8);  // (diagnostics) the wait for the slowest warp of the bi-prediction phase
           for (int d; (d = be.next(1)) < n_isearch;) intra_search_item(bi, t, d, &my_icost, &my_ik);
           be.mark(PH_INTRA_SEARCH);
         }
@@ -894,7 +946,7 @@ template <class S, class B> struct Rdo {
           be.reduce_range(&worst_cost, &best_cost);
           if (worst_cost && (uint64_t)worst_cost * 3 > (uint64_t)best_cost * 4) best_ref = 0;  // best_ref_idx is never updated in the reference (:1868, :2019)
         }
-        if (!overlap && do_bipred && do_inter) bipred_cands(bi, t, mv_center, mvp, false, &pos);
+        if (!overlap && do_bipred && do_inter) bipred_cands(bi, t, mv_center, mvp, false, &pos, JOINT_HERE);
         if (overlap && do_bipred) {  // warp 0's searches extended (and scribbled on, :873-881) the candidate lists: everybody's replica follows
           if (be.warp() != 0)
             for (int r = 0; r < F.num_ref; r++) {

@@ -2,7 +2,7 @@
 """One launch of rdo_batch_kernel over the inter frames of a captured clip, for ncu / compute-sanitizer:
   ncu --set full --import-source on --clock-control none -k regex:rdo_batch -c 1 -o rdo python tools/rdo_profile.py --size 640x384
 Prints the kernel's own counters (cycles per primitive class, work executed).  --copies 5 --size 1920x1080 is the launch bench.py times;
---trace FILE writes the per-super-block timeline of the last launch (tb_rdo_batch_trace) as .npz for tools/rdo_sched.py."""
+--trace FILE writes the per-super-block timeline of the last launch (tb_rdo_batch_trace) as .npz for tools/rdo_sched.py, with each frame's type and qp."""
 import argparse
 import ctypes as C
 import json
@@ -18,9 +18,12 @@ sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 
 # the counters behind bench.py's (include/thor_b200.h TB_RDO_NSTATS): the search phase of an overlapped block decision (tb_rdo.cu ST_X), warp 0 and the last
-# warp, each {own searches, (unused), wait at the barrier that ends the phase}
+# warp, each {own searches, (unused), wait at the barrier that ends the phase}; its bi-prediction phase (ST_XB), warp 0 {chain, inter candidates, barrier
+# wait} and the last warp {joint search as the helper, inter candidates, barrier wait}; the B-frame decisions whose joint search ran on the helper / warp 0
 SEARCH_PHASE_NAMES = ["w0_own_searches", "w0_barrier_wait", "wlast_own_searches", "wlast_barrier_wait"]
-STAT_NAMES = bench.STAT_NAMES + ["x_w0_own_searches", "x_unused_1", "x_w0_barrier_wait", "x_wlast_own_searches", "x_unused_4", "x_wlast_barrier_wait"]
+BIPRED_PHASE_NAMES = ["w0_chain", "w0_inter_cands", "w0_barrier_wait", "wlast_joint_search", "wlast_inter_cands", "wlast_barrier_wait"]
+STAT_NAMES = bench.STAT_NAMES + ["x_w0_own_searches", "x_unused_1", "x_w0_barrier_wait", "x_wlast_own_searches", "x_unused_4", "x_wlast_barrier_wait"] + \
+    ["xb_" + n for n in BIPRED_PHASE_NAMES] + ["joint_on_helper", "joint_on_warp0"]
 NSTATS = int(re.search(r"#define TB_RDO_NSTATS (\d+)", open(os.path.join(ROOT, "include", "thor_b200.h")).read()).group(1))
 assert len(STAT_NAMES) == NSTATS, (len(STAT_NAMES), NSTATS)
 
@@ -80,14 +83,18 @@ def main():
            "cycles_per_prediction": round(d["cyc_interp"] / max(1, d["predictions"])), "cycles_per_intra": round(d["cyc_intra"] / max(1, d["intra_predictions"])),
            "warp_cycles_per_super_block": round(d["cyc_total"] * (1 - d["cyc_idle"] / max(1, d["cyc_total"])) / max(1, d["super_blocks"])),
            "share": {k[4:]: round(d[k] / max(1, d["cyc_total"]), 4) for k in bench.STAT_NAMES[:10] + bench.STAT_NAMES[23:40]}, "phase": {k[3:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[40:49])), 4) for k in bench.STAT_NAMES[40:49]}, "me_stage": {k[9:]: round(d[k] / max(1, sum(d[n] for n in bench.STAT_NAMES[49:])), 4) for k in bench.STAT_NAMES[49:]}, "work": {k: d[k] for k in bench.STAT_NAMES[11:23]},
-           "search_phase_mcycles": {n: round(d["x_" + n] / 1e6) for n in SEARCH_PHASE_NAMES}}
+           "search_phase_mcycles": {n: round(d["x_" + n] / 1e6) for n in SEARCH_PHASE_NAMES},
+           "bipred_phase_mcycles": {n: round(d["xb_" + n] / 1e6) for n in BIPRED_PHASE_NAMES},
+           "joint_search": {"on_helper": d["joint_on_helper"], "on_warp0": d["joint_on_warp0"],
+                            "helper_hit_rate": round(d["joint_on_helper"] / max(1, d["joint_on_helper"] + d["joint_on_warp0"]), 4)}}
     if args.trace:
         n = L.tb_rdo_batch_trace(b, None, 0)
         tr = np.zeros(n, [(k, np.int32) for k in ("frame", "row", "col", "cta")] + [("t_start", np.uint64), ("t_end", np.uint64)])
         assert L.tb_rdo_batch_trace(b, tr.ctypes.data, n) == n, L.tb_rdo_last_error()
         sb = [1 << hf.desc.log2_sb_size for hf in hosts]
         np.savez(args.trace, **{k: tr[k] for k in tr.dtype.names}, nsbx=np.array([-(-hf.desc.width // s) for hf, s in zip(hosts, sb)]),
-                 nsby=np.array([-(-hf.desc.height // s) for hf, s in zip(hosts, sb)]), ctas=out["ctas"])
+                 nsby=np.array([-(-hf.desc.height // s) for hf, s in zip(hosts, sb)]), ctas=out["ctas"],
+                 frame_type=np.array([hf.desc.frame_type for hf in hosts]), qp=np.array([hf.desc.qp for hf in hosts]))
     print(json.dumps(out))
 
 

@@ -9,6 +9,8 @@ Reports, on the measured durations:
               blocks) and tail (after its last super block: no more work came)
   lower bound max(total super-block time / CTAs, longest dependency chain of any frame)
   longest idle stretch of any CTA, against the kernel's watchdog (6e10 SM clocks without work)
+  by frame type (traces that record each frame's type and qp): frames, qps, longest dependency chain and mean super-block time of each type,
+              which shows the frames that set the lower bound
   replay      the same durations re-scheduled by an event model of the kernel's claim rule, for several claim policies
 
 The event model: a super block (r, c) is ready when (r, c-1) and (r-1, min(c+1, nsbx-1)) have ended (row r-1 has published min(c+2, nsbx)); an idle
@@ -23,6 +25,7 @@ import numpy as np
 
 WATCHDOG_CLOCKS = 60_000_000_000  # rdo_batch_kernel: a CTA without work for this many SM clocks while work remains ends the launch
 TRACE_FIELDS = ("frame", "row", "col", "cta", "t_start", "t_end")
+FRAME_TYPES = {0: "I", 1: "P", 2: "B"}
 # index: lowest row index (frame-major); longest: longest remaining dependency path (nsbx - p) + 2 (nsby - 1 - row), ties to the lower index;
 # weighted: that path times the frame's running mean super-block time.  "-each": one super block per claim (what rdo_batch_kernel does).
 POLICIES = ("index", "longest", "longest-each", "weighted", "weighted-each")
@@ -160,6 +163,13 @@ def report(tr, sm_mhz=1980.0):
     out["launch_over_lower_bound"] = round(out["launch_s"] / lb, 4)
     sb = np.concatenate([x.reshape(-1) for x in d])
     out["super_block_s"] = {"mean": round(float(sb.mean()), 5), "cv": round(float(sb.std() / sb.mean()), 4), "min": round(float(sb.min()), 5), "max": round(float(sb.max()), 5)}
+    if "frame_type" in tr:
+        out["by_frame_type"] = {}
+        for ft in sorted(set(int(v) for v in tr["frame_type"])):
+            fs = [f for f in range(len(d)) if int(tr["frame_type"][f]) == ft]
+            out["by_frame_type"][FRAME_TYPES.get(ft, str(ft))] = {
+                "frames": len(fs), "qp": sorted(set(int(tr["qp"][f]) for f in fs)), "longest_chain_s": round(max(chains[f] for f in fs), 4),
+                "mean_super_block_s": round(float(np.concatenate([d[f].reshape(-1) for f in fs]).mean()), 5)}
     out["watchdog_s"] = round(WATCHDOG_CLOCKS / (sm_mhz * 1e6), 1)
     out["replay"] = {}
     for p in POLICIES:
