@@ -1364,7 +1364,7 @@ __device__ __forceinline__ void dot16_block(const int8_t *A, int sa, const int16
 
 // ---------------------------------------------------------------------------------------------------------------
 // a10-a13: the arithmetic rules of the transform chain.  Every chain form (the warp_* routines below, thread_txfm4,
-// thread_txfm8, tx_big_chain, DevBackend::tx_multi) keeps its own data movement and takes its stage rounding, scan
+// thread_txfm8, tx_big_chain, DevBackend::tx_small / tx_mid) keeps its own data movement and takes its stage rounding, scan
 // order, quantiser and dequantiser from here.
 // ---------------------------------------------------------------------------------------------------------------
 __constant__ uint16_t c_quant[6] = {26214, 23302, 20560, 18396, 16384, 14564};  // common/common_tables.c:72
@@ -1518,18 +1518,14 @@ __device__ void warp_inv_transform(const int16_t *coef, int cpitch, int size, in
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// a12: quantize.  enc/encode_block.c:84-160.  coef: compact qsize x qsize (raster).  The level_mode hysteresis is a
-// two-state machine along the zig-zag scan; each lane simulates its 8-position chunk for both start states, a warp
-// scan composes the state maps, then each lane replays its chunk from the true start state.
+// a12: quantize.  enc/encode_block.c:84-160.  The level_mode hysteresis is a two-state machine along the zig-zag scan;
+// each lane simulates its 8-position chunk for both start states, a warp scan composes the state maps, then each lane
+// replays its chunk from the true start state.
+// warp_quantize_scan: nq (<= 256) coefficients already in scan order -> their signed levels in scan order.  lev may be
+// scan itself: every lane writes only the positions it read.  Returns cbp (any level != 0) on every lane.
 // ---------------------------------------------------------------------------------------------------------------
-__device__ int warp_quantize(const int16_t *coef, int16_t *coefq, int qp, int size, int coeff_type, TxScratch &sc, const uint8_t *zz16 = nullptr) {
+__device__ int warp_quantize_scan(const int16_t *scan, int16_t *lev, int nq, const Quantizer &Q) {
   const int lane = lane_id();
-  const int qsize = min(size, 16), nq = qsize * qsize, lq = ilog2(qsize);
-  const Quantizer Q(qp, ilog2(size), coeff_type);
-  int *scan = (int *)sc.in;  // reuse: 256 ints of scan-ordered coefficients
-  const bool tab = zz16 != nullptr && qsize == 16;  // 16x16 scan positions from a shared-memory table instead of the closed form
-  for (int p = lane; p < nq; p += 32) scan[tab ? (int)zz16[p] : zigzag_index(p >> lq, p & (qsize - 1), qsize)] = coef[p];
-  __syncwarp();
   // each lane owns `per` (<= 8) consecutive scan positions; their levels in both level modes are computed ONCE and kept in registers
   const int per = (nq + 31) / 32, p0 = lane * per;
   int cv[8], lv0[8], lv1[8];
@@ -1576,13 +1572,24 @@ __device__ int warp_quantize(const int16_t *coef, int16_t *coefq, int qp, int si
         cbp |= level != 0;
         mode = Quantizer::next_mode(mode, level);
       }
-      sc.tmp[p] = (int16_t)q;  // scan order
+      lev[p] = (int16_t)q;  // scan order
     }
   }
   __syncwarp();
+  return __any_sync(FULL, cbp);
+}
+// coef: compact qsize x qsize (raster) -> coefq (raster); the levels stay in sc.tmp in scan order
+__device__ int warp_quantize(const int16_t *coef, int16_t *coefq, int qp, int size, int coeff_type, TxScratch &sc, const uint8_t *zz16 = nullptr) {
+  const int lane = lane_id();
+  const int qsize = min(size, 16), nq = qsize * qsize, lq = ilog2(qsize);
+  int16_t *scan = sc.in;  // reuse: the coefficients in scan order
+  const bool tab = zz16 != nullptr && qsize == 16;  // 16x16 scan positions from a shared-memory table instead of the closed form
+  for (int p = lane; p < nq; p += 32) scan[tab ? (int)zz16[p] : zigzag_index(p >> lq, p & (qsize - 1), qsize)] = coef[p];
+  __syncwarp();
+  const int cbp = warp_quantize_scan(scan, sc.tmp, nq, Quantizer(qp, ilog2(size), coeff_type));
   for (int p = lane; p < nq; p += 32) coefq[p] = sc.tmp[tab ? (int)zz16[p] : zigzag_index(p >> lq, p & (qsize - 1), qsize)];
   __syncwarp();
-  return __any_sync(FULL, cbp);
+  return cbp;
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -73,13 +73,20 @@ struct RdoCta {
   unsigned long long t_sb;  // %globaltimer when the current super block started
 };
 // per-warp scratch
+constexpr int TX_TILES = 3584;  // int16 tiles of the 16x16 / 32x32 chains (tx_mid), in the space of the other transform forms' scratch
 template <class S> struct RdoShared {
   long long prof[ST_END];
   long long t_mark, t_mark2;
   alignas(16) unsigned char jobs[12 * 64];  // tx_multi: the chains' parameters
-  TxScratch sc;
-  alignas(16) int16_t blk16[256];                // early skip: averaged residual / chroma residual
-  alignas(16) int16_t out16[256];                // transform output of the early-skip test; coefficient scan for the bit count
+  union {
+    struct {
+      TxScratch sc;
+      alignas(16) int16_t blk16[256];            // early skip: averaged residual / chroma residual
+      alignas(16) int16_t out16[256];            // transform output of the early-skip test; coefficient scan for the bit count
+    };
+    alignas(16) int16_t tiles[TX_TILES];
+  };
+  static_assert(TX_TILES * sizeof(int16_t) <= sizeof(TxScratch) + 2 * 256 * sizeof(int16_t), "the tiles take no shared memory of their own");
   alignas(16) S left[256], top[256], filt[4 * 128 + 4];
   tb_txfm_result_t res;
 };
@@ -275,30 +282,143 @@ template <class S> struct DevBackend {
     sync();
   }
   __device__ __noinline__ int tx_chain(const S *orig, int os, const S *pred, int ps, S *rec, int rs, int16_t *cq, int size, int qp, int coeff_type, int fast) const {
+    tbr::TxJob<S> j;
+    j.orig = orig; j.pred = pred; j.rec = rec; j.cq = cq; j.os = os; j.ps = ps; j.rs = rs; j.size = size; j.qp = qp; j.coeff_type = coeff_type; j.fast = fast;
     int cbp;
-    if (size < 16) {  // 4x4 / 8x8: the loop form below, one chain
-      tbr::TxJob<S> j;
-      j.orig = orig; j.pred = pred; j.rec = rec; j.cq = cq; j.os = os; j.ps = ps; j.rs = rs; j.size = size; j.qp = qp; j.coeff_type = coeff_type; j.fast = fast;
-      tx_multi(&j, 1, &cbp);
-      return cbp;
-    }
-    PROF2(PF_TX, ST_TX_SZ + ilog2(size) - 2);
-    if (lane() == 0) { sh->prof[ST_TX] += 1; sh->prof[ST_TX_SAMPLES] += 3 * size * size; }
+    tx_multi(&j, 1, &cbp);
+    return cbp;
+  }
+  // chains of one transform size (4x4 and 8x8 may mix), in the order of the list; bit[k] = cbp of chain k
+  __device__ __noinline__ void tx_multi(const tbr::TxJob<S> *jobs, int n, int *bit) const {
+    if (jobs[0].size <= 8) tx_small(jobs, n, bit);
+    else if (jobs[0].size <= 32) tx_mid(jobs, n, bit);
+    else
+      TB_ROLL
+      for (int k = 0; k < n; k++) bit[k] = tx_big(jobs[k]);
+  }
+  // 64x64 / 128x128: the CTA kernels' chain (tb_kernels.cuh) on this warp
+  __device__ __noinline__ int tx_big(const tbr::TxJob<S> &j) const {
+    PROF2(PF_TX, ST_TX_SZ + ilog2(j.size) - 2);
+    if (lane() == 0) { sh->prof[ST_TX] += 1; sh->prof[ST_TX_SAMPLES] += 3 * j.size * j.size; }
     sync();
     tb_txfm_item_t q;
-    q.orig = orig; q.pred = pred; q.rec = rec; q.coeffq = cq; q.ostride = os; q.pstride = ps; q.rstride = rs;
-    q.size = (uint8_t)size; q.qp = (uint8_t)qp; q.coeff_type = (uint8_t)coeff_type; q.fast = (uint8_t)(fast ? TB_TXFM_FAST : 0);
+    q.orig = j.orig; q.pred = j.pred; q.rec = j.rec; q.coeffq = j.cq; q.ostride = j.os; q.pstride = j.ps; q.rstride = j.rs;
+    q.size = (uint8_t)j.size; q.qp = (uint8_t)j.qp; q.coeff_type = (uint8_t)j.coeff_type; q.fast = (uint8_t)(j.fast ? TB_TXFM_FAST : 0);
     tx_big_chain<S, 1>(q, F->bitdepth, sh->sc, nullptr, cta->tab8, cta->tab8 + DCT_TAB8_SIZE, nullptr, nullptr, &sh->res);
     sync();
-    cbp = sh->res.cbp;
+    const int cbp = sh->res.cbp;
     sync();
     return cbp;
+  }
+  // m . v over 16 * nc terms (int8 matrix row, int16 vector; both 16-byte aligned)
+  __device__ __forceinline__ static int dot_rows(const int8_t *m, const int16_t *v, int nc) {
+    int acc[1][1] = {{0}};
+    TB_ROLL
+    for (int c = 0; c < nc; c++) dot16_block<1, 1>(m + 16 * c, 0, v + 16 * c, 0, acc);
+    return acc[0][0];
+  }
+  // <= 12 chains of 16x16 or 32x32 transform blocks, all of the same size and `fast` flag: 32x32 is the 32-point forward transform (or, with `fast`,
+  // the 16-point one on the 2x2 box sums of the residual, which wrap in int16 as transform_simd's do), 16x16 coefficients and the 32-point inverse
+  // core.  The arithmetic of tx_big_chain; written, like tx_small, as LOOPS over (chain, element) work items dealt to the lanes, one output per item
+  // with the 16-term DP2A dot product of dot16_block, so that the code stays a few KB.  The chains of a group share every stage: four of 16x16 or of
+  // 32x32 with `fast`, one of 32x32 without it, in the TX_TILES int16 of the warp's scratch.  Per chain two tiles:
+  //   X: residual (s1 x s1, pitch p1) -> coefficients in scan order, quantised in place (256) -> inverse first stage, transposed (N x 16)
+  //   Y: forward first stage (16 x s1, pitch p1) -> dequantised coefficients, transposed (16 x 16, pitch 24)
+  // Pitches of tiles whose rows the lanes of a quarter-warp read side by side are 48 or 80 bytes: conflict-free 128-bit loads.  The quantiser's
+  // level-mode walk stays warp-parallel (warp_quantize_scan), one chain after the other.
+  __device__ __noinline__ void tx_mid(const tbr::TxJob<S> *jobs, int n, int *bit) const {
+    const int N = jobs[0].size, ln = ilog2(N), l1 = (N == 32 && jobs[0].fast) ? 4 : ln, s1 = 1 << l1, p1 = s1 + 8;
+    PROF2(PF_TX, ST_TX_SZ + ln - 2);
+    const int l = lane();
+    if (l == 0) { sh->prof[ST_TX] += n; sh->prof[ST_TX_SAMPLES] += 3 * n * N * N; }
+    tbr::TxJob<S> *J = (tbr::TxJob<S> *)sh->jobs;
+    sync();
+    if (l < n) J[l] = jobs[l];
+    sync();
+    const int xs = max(s1 * p1, N * 16), cs = xs + 16 * p1, g = TX_TILES / cs;
+    const int bd = F->bitdepth, maxv = (1 << bd) - 1;
+    const int8_t *M1 = cta->tab8 + dct_tab8_ofs(l1), *Mt = cta->tab8 + DCT_TAB8_SIZE + dct_tab8_ofs(ln);
+    const uint8_t *zz16 = (const uint8_t *)(cta->tab8 + 2 * DCT_TAB8_SIZE);
+    const FwdRound R(ln, ln - l1, bd);
+    const InvRound RI(bd);
+    int16_t *T = sh->tiles;
+    TB_ROLL
+    for (int k0 = 0; k0 < n; k0 += g) {
+      const int m = min(g, n - k0);
+      const tbr::TxJob<S> *G = J + k0;
+      // (1) residual -> X[k][i][j]; with `fast` the 2x2 box sums
+      TB_ROLL
+      for (int w = l; w < (m << (2 * l1)); w += 32) {
+        const int k = w >> (2 * l1), e = w & ((1 << (2 * l1)) - 1), i = e >> l1, j = e & (s1 - 1);
+        const tbr::TxJob<S> &q = G[k];
+        int v = 0;
+        if (l1 == ln) v = (int)q.orig[i * q.os + j] - (int)q.pred[i * q.ps + j];
+        else
+          TB_ROLL
+          for (int t = 0; t < 4; t++) {
+            const int y = 2 * i + (t >> 1), x = 2 * j + (t & 1);
+            v += (int)q.orig[y * q.os + x] - (int)q.pred[y * q.ps + x];
+          }
+        T[k * cs + i * p1 + j] = (int16_t)v;  // modulo 2^16
+      }
+      sync();
+      // (2) forward, first dimension: Y[k][i][j] = stage1(M[i][.] . X[k][j][.])   (i < 16, j < s1)
+      TB_ROLL
+      for (int w = l; w < (m << (4 + l1)); w += 32) {
+        const int k = w >> (4 + l1), e = w & ((16 << l1) - 1), i = e >> l1, j = e & (s1 - 1);
+        T[k * cs + xs + i * p1 + j] = (int16_t)R.stage1(dot_rows(M1 + (i << l1), T + k * cs + j * p1, s1 >> 4));
+      }
+      sync();
+      // (3) forward, second dimension, to X[k] in scan order: X[k][zz(i, j)] = stage2(M[i][.] . Y[k][j][.])   (i, j < 16)
+      TB_ROLL
+      for (int w = l; w < (m << 8); w += 32) {
+        const int k = w >> 8, e = w & 255, i = e >> 4, j = e & 15;
+        T[k * cs + zz16[e]] = (int16_t)R.stage2(dot_rows(M1 + (i << l1), T + k * cs + xs + j * p1, s1 >> 4));
+      }
+      sync();
+      // (4) quantiser, in place, one chain after the other
+      unsigned nz = 0;
+      TB_ROLL
+      for (int k = 0; k < m; k++) {
+        const tbr::TxJob<S> &q = G[k];
+        nz |= (unsigned)warp_quantize_scan(T + k * cs, T + k * cs, 256, Quantizer(q.qp, ln, q.coeff_type)) << k;
+      }
+      // (5) levels, raster, to the caller's buffer (reference layout) and, dequantised, transposed to Y[k][j][i] = rcoeff[i][j] (pitch 24)
+      TB_ROLL
+      for (int w = l; w < (m << 8); w += 32) {
+        const int k = w >> 8, e = w & 255;
+        const tbr::TxJob<S> &q = G[k];
+        const int c = T[k * cs + zz16[e]];
+        q.cq[e] = (int16_t)c;
+        T[k * cs + xs + (e & 15) * 24 + (e >> 4)] = (int16_t)Dequantizer(q.qp, ln)(c);
+      }
+      sync();
+      // (6) inverse, first dimension: X[k][j][i] = stage1(sum_t M[t][j] * rcoeff[t][i])   (j < N, i < 16; pitch 16)
+      TB_ROLL
+      for (int w = l; w < (m << (ln + 4)); w += 32) {
+        const int k = w >> (ln + 4), e = w & ((16 << ln) - 1), j = e >> 4, i = e & 15;
+        if ((nz >> k) & 1) T[k * cs + e] = (int16_t)InvRound::stage1(dot_rows(Mt + (j << ln), T + k * cs + xs + i * 24, 1));
+      }
+      sync();
+      // (7) inverse, second dimension + reconstruction: rec = clip(pred + stage2(sum_t M[t][j] * X[k][i][t])); no coefficient: rec = pred
+      TB_ROLL
+      for (int w = l; w < (m << (2 * ln)); w += 32) {
+        const int k = w >> (2 * ln), e = w & ((1 << (2 * ln)) - 1), i = e >> ln, j = e & (N - 1);
+        const tbr::TxJob<S> &q = G[k];
+        int v = (int)q.pred[i * q.ps + j];
+        if ((nz >> k) & 1) v = sat_px(v + RI.stage2(dot_rows(Mt + (j << ln), T + k * cs + i * 16, 1)), maxv);
+        q.rec[i * q.rs + j] = (S)v;
+      }
+      sync();
+      TB_ROLL
+      for (int k = 0; k < m; k++) bit[k0 + k] = (nz >> k) & 1;
+    }
   }
   // <= 12 chains of 4x4 / 8x8 transform blocks (residual -> DCT -> quantiser -> dequantiser -> inverse DCT -> reconstruction, the arithmetic of
   // common/transform.c:245-308, 411-494, enc/encode_block.c:84-171, common/common_block.c:45-83), all of them together on the warp.  Written as LOOPS over
   // (chain, element) work items dealt to the lanes: the RD loop is bound by instruction fetch, so a few hundred instructions that stay in the instruction cache beat the unrolled one-thread-per-chain forms (5.6 k instructions
   // streamed from L2 per call).  Tiles of 64 int16 per chain in the warp's scratch; the quantiser's level-mode walk is sequential: one lane per chain.
-  __device__ __noinline__ void tx_multi(const tbr::TxJob<S> *jobs, int n, int *bit) const {
+  __device__ __noinline__ void tx_small(const tbr::TxJob<S> *jobs, int n, int *bit) const {
     PROF2(PF_TX, ST_TX_SZ + ilog2(jobs[0].size) - 2);
     const int l = lane();
     if (l == 0)

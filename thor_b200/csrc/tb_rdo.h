@@ -460,21 +460,6 @@ template <class S, class B> struct Rdo {
     q.fast = inter_fast(size, 0);
     return 1;
   }
-  // encode_and_reconstruct_block_inter for one plane: the chains of inter_jobs one after the other, without the job list; returns the cbp
-  TBR_HD TBR_NI int enc_rec_inter(const S *orig, int os, int size, int qp, const S *pred, int16_t *cq, S *rec, int coeff_type, int tb_split) {
-    if (tb_split) {
-      const int s2 = size / 2;
-      int cbp = 0, index = 0;
-      for (int i = 0; i < size; i += s2)
-        for (int j = 0; j < size; j += s2) {
-          const int bit = be.tx_chain(orig + i * os + j, os, pred + i * size + j, size, rec + i * size + j, size, cq + index, s2, qp, coeff_type, inter_fast(size, 1));
-          cbp = (cbp << 1) + bit;
-          index += 256;
-        }
-      return cbp;
-    }
-    return be.tx_chain(orig, os, pred, size, rec, size, cq, size, qp, coeff_type, inter_fast(size, 0));
-  }
   TBR_HD static int join_cbp(const int *bit, int n) {
     int cbp = 0;
     for (int k = 0; k < n; k++) cbp = (cbp << 1) + bit[k];
@@ -499,10 +484,10 @@ template <class S, class B> struct Rdo {
     be.intra_predict(pblock, size, recf, rfs, (const S *)nullptr, 0, 0, 0, ypos, xpos, size, upright, downleft, 0, intra_mode);
     return be.tx_chain(orig, os, pblock, size, rec_block, size, cq, size, qp, coeff_type, fast);
   }
-  // the U and the V chain of one transform block: independent, side by side when they are thread-sized (<= 8x8)
+  // the U and the V chain of one transform block: independent, side by side up to 16x16
   TBR_HD TBR_NI void uv_chains(const S *ou, const S *ov, int os, const S *pu, const S *pv, int ps, S *ru, S *rv, int rs, int16_t *cqu, int16_t *cqv, int size, int qp, int coeff_type,
                         int fast, int *bu, int *bv) {
-    if (size <= 8) {
+    if (size <= 16) {
       TxJob<S> jobs[2];
       int bit[2];
       jobs[0].orig = ou; jobs[0].pred = pu; jobs[0].rec = ru; jobs[0].cq = cqu; jobs[1].orig = ov; jobs[1].pred = pv; jobs[1].rec = rv; jobs[1].cq = cqv;
@@ -569,12 +554,13 @@ template <class S, class B> struct Rdo {
         be.copy(W.rec_v, sizeC, W.p_v, sizeC, sizeC, sizeC);
         c.cbp_y = c.cbp_u = c.cbp_v = 0;
       } else {
+        TxJob<S> jobs[12];
+        int bit[12];
         if (!F.cfl_inter && sizeC <= 8) {
           // small blocks: the chains of the three planes (<= 12 of 4x4 / 8x8, one thread each on the device) side by side; a 16x16 luma block goes first, alone
-          TxJob<S> jobs[12];
-          int bit[12], n = 0, ny = 0;
+          int n = 0, ny = 0;
           const int tbc = tb_split && sizeC > 4;
-          if (size == 16 && !tb_split) c.cbp_y = enc_rec_inter(oy, F.org_stride[0], size, F.qp, W.p_y, W.cq_y, W.rec_y, itype | 0, 0);
+          if (size == 16 && !tb_split) c.cbp_y = be.tx_chain(oy, F.org_stride[0], W.p_y, size, W.rec_y, size, W.cq_y, size, F.qp, itype | 0, inter_fast(size, 0));
           else { ny = inter_jobs(jobs, oy, F.org_stride[0], size, F.qp, W.p_y, W.cq_y, W.rec_y, itype | 0, tb_split); n = ny; }
           const int nu = inter_jobs(jobs + n, ou, F.org_stride[1], sizeC, F.qpc, W.p_u, W.cq_u, W.rec_u, itype | 1, tbc);
           n += nu;
@@ -585,10 +571,17 @@ template <class S, class B> struct Rdo {
           c.cbp_u = join_cbp(bit + ny, nu);
           c.cbp_v = join_cbp(bit + ny + nu, nv);
         } else {
-          c.cbp_y = enc_rec_inter(oy, F.org_stride[0], size, F.qp, W.p_y, W.cq_y, W.rec_y, itype | 0, tb_split);
+          // one plane after the other (CfL predicts chroma from the luma reconstruction), the transform blocks of a plane side by side
+          int n = inter_jobs(jobs, oy, F.org_stride[0], size, F.qp, W.p_y, W.cq_y, W.rec_y, itype | 0, tb_split);
+          be.tx_multi(jobs, n, bit);
+          c.cbp_y = join_cbp(bit, n);
           if (F.cfl_inter) be.cfl(W.p_y, W.p_u, W.p_v, W.rec_y, size, size, size);
-          c.cbp_u = enc_rec_inter(ou, F.org_stride[1], sizeC, F.qpc, W.p_u, W.cq_u, W.rec_u, itype | 1, tb_split && sizeC > 4);
-          c.cbp_v = enc_rec_inter(ov, F.org_stride[1], sizeC, F.qpc, W.p_v, W.cq_v, W.rec_v, itype | 1, tb_split && sizeC > 4);
+          n = inter_jobs(jobs, ou, F.org_stride[1], sizeC, F.qpc, W.p_u, W.cq_u, W.rec_u, itype | 1, tb_split && sizeC > 4);
+          be.tx_multi(jobs, n, bit);
+          c.cbp_u = join_cbp(bit, n);
+          n = inter_jobs(jobs, ov, F.org_stride[1], sizeC, F.qpc, W.p_v, W.cq_v, W.rec_v, itype | 1, tb_split && sizeC > 4);
+          be.tx_multi(jobs, n, bit);
+          c.cbp_v = join_cbp(bit, n);
         }
       }
     }
