@@ -105,7 +105,9 @@ CASES = [
     # 8916 / 8658 4x4 cells from wholly outside the picture (split_mv's clamps)
     ("hdb_pan_neg",      HDB0,                                                         384, 256, 9, 32, 8,  "pan_neg"),
     ("hdb_pan_pos",      HDB0,                                                         384, 256, 9, 32, 8,  "pan_pos"),
-    # 12 bits: box sums of 16 residuals leave int16 (128x128 transforms wrap), the inverse transform's second stage can saturate
+    # 12 bits: box sums of 16 residuals leave int16, the inverse transform's second stage can saturate.  The 4x4 box sums wrap in some 128x128
+    # chains of hdb_q4_hard_12 and hdb_q32_hard_12 and saturate in some 64x64 chains with `fast` of speed1_hard_12.  No one case can do both:
+    # speed 0 runs no 64x64 chain with `fast`, speeds 1 and up no 128x128 chain (enc/encode_block.c:1298, 1319, 1912).
     ("hdb_q51_12",       HDB0,                                                         128, 136, 5, 51, 12, "synth"),
     ("hdb_q4_hard_12",   HDB0,                                                         128, 136, 5, 4,  12, "hard"),
     ("hdb_q32_hard_12",  HDB0,                                                         128, 136, 5, 32, 12, "hard"),

@@ -1306,6 +1306,7 @@ constexpr int DCT_TAB_SIZE = 1360;
 __device__ __forceinline__ int dct_tab_ofs(int lN) { return lN == 2 ? 0 : (lN == 3 ? 16 : (lN == 4 ? 80 : 336)); }
 // int8 tables, natural pitches: the 16/32-point rows are read with 128-bit loads that are uniform per quarter-warp (dot16_block)
 constexpr int DCT_TAB8_SIZE = 16 + 64 + 16 * 16 + 32 * 32;  // 1360; every row of the 16- and 32-point tables is 16-byte aligned
+constexpr int TX_TABLE_BYTES = (DCT_TAB8_SIZE * 2 + 256 + 15) & ~15;  // int8 matrices (plain, transposed) + 16x16 zig-zag table
 __device__ __forceinline__ int dct_tab8_ofs(int lN) { return lN == 2 ? 0 : (lN == 3 ? 16 : (lN == 4 ? 80 : 336)); }
 __device__ __forceinline__ int dct_tab8_pitch(int lN) { return 1 << lN; }
 __device__ __forceinline__ void dct_tab_fill(int16_t *tab) {  // call with all threads of the CTA, then __syncthreads()
@@ -1364,8 +1365,8 @@ __device__ __forceinline__ void dot16_block(const int8_t *A, int sa, const int16
 
 // ---------------------------------------------------------------------------------------------------------------
 // a10-a13: the arithmetic rules of the transform chain.  Every chain form (the warp_* routines below, thread_txfm4,
-// thread_txfm8, tx_big_chain, DevBackend::tx_small / tx_mid) keeps its own data movement and takes its stage rounding, scan
-// order, quantiser and dequantiser from here.
+// thread_txfm8, tx_big_chain, DevBackend::tx_small / tx_mid) keeps its own data movement and takes its box sums, stage
+// rounding, scan order, quantiser and dequantiser from here.
 // ---------------------------------------------------------------------------------------------------------------
 __constant__ uint16_t c_quant[6] = {26214, 23302, 20560, 18396, 16384, 14564};  // common/common_tables.c:72
 __constant__ uint16_t c_dequant[6] = {40, 45, 51, 57, 64, 72};                  // common/common_tables.c:73
@@ -1384,6 +1385,30 @@ template <int N> struct ZigZag {
   uint8_t pos[N * N];
   __host__ __device__ constexpr ZigZag() : pos() {
     for (int p = 0; p < N * N; p++) pos[p] = (uint8_t)zigzag_index(p / N, p % N, N);
+  }
+};
+
+// Input of the forward transform, as transform_simd forms it (common/common_kernels.c:1482-1549): a size x size residual larger
+// than 32 >> fast becomes size1 x size1 box sums of scale x scale residuals, added rows outer, columns inner.  64x64 and 128x128
+// with `fast` saturate to [-16384, 16383] after every addition (:1524-1529); every other box sum wraps in int16 (:1501-1503,
+// :1544-1549), which the low 16 bits of the int sum give.  Saturating every box sum would differ only for 128x128 without `fast`
+// above 10 bits: a partial sum of 4 residuals stays within [-16384, 16383] at every bit depth (4 x 4095 = 16380), one of 16
+// residuals up to 10 bits (16 x 1023 = 16368).
+struct BoxSum {
+  int size1, log2scale;
+  bool sat;
+  __device__ __forceinline__ BoxSum(int size, int fast)
+      : size1(min(size, 32 >> fast)), log2scale(ilog2(size) - ilog2(min(size, 32 >> fast))), sat(fast && size >= 64) {}
+  __device__ __forceinline__ int scale() const { return 1 << log2scale; }
+  // partial sum + the next residual
+  __device__ __forceinline__ int add(int sum, int r) const { sum += r; return sat ? iclip(sum, -16384, 16383) : sum; }
+  // transform input (i, j) from the residual res(y, x)
+  template <class R> __device__ __forceinline__ int16_t operator()(int i, int j, R res) const {
+    const int s = scale();
+    int sum = 0;
+    TB_ROLL
+    for (int t = 0; t < s * s; t++) sum = add(sum, res(i * s + (t >> log2scale), j * s + (t & (s - 1))));
+    return (int16_t)sum;
   }
 };
 
@@ -1444,31 +1469,15 @@ struct alignas(16) TxScratch {
 // compact qsize x qsize output `coef` (pitch qsize).  Returns nothing; all lanes participate.
 __device__ void warp_fwd_transform(const int16_t *block, int bpitch, int size, int fast, int bitdepth, TxScratch &sc, int16_t *coef, const int16_t *tab) {
   const int lane = lane_id();
-  int size1 = size, scale = 1;
-  if (size > (32 >> fast)) { size1 = 32 >> fast; scale = size / size1; }
-  const int l1 = ilog2(size1), qsize = min(size, 16);
+  const BoxSum B(size, fast);
+  const int size1 = B.size1, l1 = ilog2(size1), qsize = min(size, 16);
   const int16_t *M = tab + dct_tab_ofs(l1);
-  // load, with the box sum of large blocks formed as transform_simd forms it: 64x64 and 128x128 with `fast` saturate after every
-  // addition (common/common_kernels.c:1524-1529), every other box sum wraps in int16 (:1501-1503, :1544-1549).  The rules differ only
-  // for 128x128 without `fast` above 10 bits: no partial sum of at most 16 residuals of 10 bits or fewer leaves [-16384, 16383].
-  const bool sat = fast && size >= 64;
   for (int p = lane; p < size1 * size1; p += 32) {
     int i = p >> l1, j = p & (size1 - 1);
-    int v;
-    if (scale == 1) v = block[i * bpitch + j];
-    else {
-      int sum = 0;
-      for (int m = 0; m < scale; m++)
-        for (int n = 0; n < scale; n++) {
-          sum += block[(i * scale + m) * bpitch + j * scale + n];
-          if (sat) sum = iclip(sum, -16384, 16383);
-        }
-      v = sum;
-    }
-    sc.in[i * 33 + j] = (int16_t)v;  // modulo 2^16
+    sc.in[i * 33 + j] = B(i, j, [&](int y, int x) { return (int)block[y * bpitch + x]; });
   }
   __syncwarp();
-  const FwdRound R(ilog2(size), ilog2(scale), bitdepth);
+  const FwdRound R(ilog2(size), B.log2scale, bitdepth);
   // 1st dimension: tmp[i][j] = stage1(sum_k M[i][k] * in[j][k]), i < qsize, j < size1
   for (int p = lane; p < qsize * size1; p += 32) {
     int i = p >> l1, j = p & (size1 - 1);

@@ -5,8 +5,9 @@
 // has published c+2 super blocks: left, up-left, up, up-right neighbours; frames are independent) — and downloads the decisions
 // (reconstruction, per-4x4 block state, the leaf list of every super block with its coefficients).
 // The control flow is tb_rdo.h (shared with the CPU host check that pins it against the reference); this file supplies its backend:
-// the warp-cooperative primitives of tb_device.cuh / tb_kernels.cuh, i.e. the same device routines the batched tb_* entry points
-// and the drop-in symbols use (parity-tested against the oracle one by one in tests/test_gpu_parity.py).
+// the warp-cooperative primitives of tb_device.cuh, the same device routines the batched tb_* entry points and the drop-in symbols
+// use (parity-tested against the oracle one by one in tests/test_gpu_parity.py), and the RD loop's own loop forms of the transform
+// chain (tx_small, tx_mid), which take their arithmetic from the same a10-a13 rules.
 //
 // This is a separate translation unit because two load policies differ from the batched kernels:
 //   TB_LDG -> plain load: the "original" of a search can be a scratch block this CTA wrote a moment ago (bipred target 2*org - pred),
@@ -24,7 +25,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <cmath>
-#include "tb_kernels.cuh"
+#include "tb_device.cuh"
 #include "tb_rdo.h"
 
 using namespace tb;
@@ -73,7 +74,7 @@ struct RdoCta {
   unsigned long long t_sb;  // %globaltimer when the current super block started
 };
 // per-warp scratch
-constexpr int TX_TILES = 3584;  // int16 tiles of the 16x16 / 32x32 chains (tx_mid), in the space of the other transform forms' scratch
+constexpr int TX_TILES = 3584;  // int16 tiles of the 16x16 to 128x128 chains (tx_mid), in the space of the other transform forms' scratch
 template <class S> struct RdoShared {
   long long prof[ST_END];
   long long t_mark, t_mark2;
@@ -88,7 +89,6 @@ template <class S> struct RdoShared {
   };
   static_assert(TX_TILES * sizeof(int16_t) <= sizeof(TxScratch) + 2 * 256 * sizeof(int16_t), "the tiles take no shared memory of their own");
   alignas(16) S left[256], top[256], filt[4 * 128 + 4];
-  tb_txfm_result_t res;
 };
 
 template <class S> struct DevBackend {
@@ -291,24 +291,7 @@ template <class S> struct DevBackend {
   // chains of one transform size (4x4 and 8x8 may mix), in the order of the list; bit[k] = cbp of chain k
   __device__ __noinline__ void tx_multi(const tbr::TxJob<S> *jobs, int n, int *bit) const {
     if (jobs[0].size <= 8) tx_small(jobs, n, bit);
-    else if (jobs[0].size <= 32) tx_mid(jobs, n, bit);
-    else
-      TB_ROLL
-      for (int k = 0; k < n; k++) bit[k] = tx_big(jobs[k]);
-  }
-  // 64x64 / 128x128: the CTA kernels' chain (tb_kernels.cuh) on this warp
-  __device__ __noinline__ int tx_big(const tbr::TxJob<S> &j) const {
-    PROF2(PF_TX, ST_TX_SZ + ilog2(j.size) - 2);
-    if (lane() == 0) { sh->prof[ST_TX] += 1; sh->prof[ST_TX_SAMPLES] += 3 * j.size * j.size; }
-    sync();
-    tb_txfm_item_t q;
-    q.orig = j.orig; q.pred = j.pred; q.rec = j.rec; q.coeffq = j.cq; q.ostride = j.os; q.pstride = j.ps; q.rstride = j.rs;
-    q.size = (uint8_t)j.size; q.qp = (uint8_t)j.qp; q.coeff_type = (uint8_t)j.coeff_type; q.fast = (uint8_t)(j.fast ? TB_TXFM_FAST : 0);
-    tx_big_chain<S, 1>(q, F->bitdepth, sh->sc, nullptr, cta->tab8, cta->tab8 + DCT_TAB8_SIZE, nullptr, nullptr, &sh->res);
-    sync();
-    const int cbp = sh->res.cbp;
-    sync();
-    return cbp;
+    else tx_mid(jobs, n, bit);
   }
   // m . v over 16 * nc terms (int8 matrix row, int16 vector; both 16-byte aligned)
   __device__ __forceinline__ static int dot_rows(const int8_t *m, const int16_t *v, int nc) {
@@ -317,17 +300,19 @@ template <class S> struct DevBackend {
     for (int c = 0; c < nc; c++) dot16_block<1, 1>(m + 16 * c, 0, v + 16 * c, 0, acc);
     return acc[0][0];
   }
-  // <= 12 chains of 16x16 or 32x32 transform blocks, all of the same size and `fast` flag: 32x32 is the 32-point forward transform (or, with `fast`,
-  // the 16-point one on the 2x2 box sums of the residual, which wrap in int16 as transform_simd's do), 16x16 coefficients and the 32-point inverse
-  // core.  The arithmetic of tx_big_chain; written, like tx_small, as LOOPS over (chain, element) work items dealt to the lanes, one output per item
-  // with the 16-term DP2A dot product of dot16_block, so that the code stays a few KB.  The chains of a group share every stage: four of 16x16 or of
-  // 32x32 with `fast`, one of 32x32 without it, in the TX_TILES int16 of the warp's scratch.  Per chain two tiles:
-  //   X: residual (s1 x s1, pitch p1) -> coefficients in scan order, quantised in place (256) -> inverse first stage, transposed (N x 16)
+  // <= 12 chains of 16x16 to 128x128 transform blocks, all of the same size and `fast` flag: the 16- or 32-point forward transform of the s1 x s1
+  // box sums of the residual (BoxSum), 16x16 coefficients, and the inverse on a core of min(N, 32) points whose every output a block larger than
+  // 32x32 replicates rep x rep (common/transform.c:481-492).  Written, like tx_small, as LOOPS over (chain, element) work items dealt to the lanes,
+  // one output per item with the 16-term DP2A dot product of dot16_block, so that the code stays a few KB.  The chains of a group share every
+  // stage: four with s1 = 16 (16x16, and every size with `fast`), one with s1 = 32, in the TX_TILES int16 of the warp's scratch.  Per chain two tiles:
+  //   X: box sums (s1 x s1, pitch p1) -> coefficients in scan order, quantised in place (256) -> inverse first stage, transposed (core x 16)
   //   Y: forward first stage (16 x s1, pitch p1) -> dequantised coefficients, transposed (16 x 16, pitch 24)
   // Pitches of tiles whose rows the lanes of a quarter-warp read side by side are 48 or 80 bytes: conflict-free 128-bit loads.  The quantiser's
   // level-mode walk stays warp-parallel (warp_quantize_scan), one chain after the other.
   __device__ __noinline__ void tx_mid(const tbr::TxJob<S> *jobs, int n, int *bit) const {
-    const int N = jobs[0].size, ln = ilog2(N), l1 = (N == 32 && jobs[0].fast) ? 4 : ln, s1 = 1 << l1, p1 = s1 + 8;
+    const int N = jobs[0].size, ln = ilog2(N);
+    const BoxSum B(N, jobs[0].fast);
+    const int s1 = B.size1, l1 = ilog2(s1), p1 = s1 + 8, core = min(N, 32), lc = ilog2(core), lr = ln - lc;
     PROF2(PF_TX, ST_TX_SZ + ln - 2);
     const int l = lane();
     if (l == 0) { sh->prof[ST_TX] += n; sh->prof[ST_TX_SAMPLES] += 3 * n * N * N; }
@@ -335,31 +320,23 @@ template <class S> struct DevBackend {
     sync();
     if (l < n) J[l] = jobs[l];
     sync();
-    const int xs = max(s1 * p1, N * 16), cs = xs + 16 * p1, g = TX_TILES / cs;
+    const int xs = max(s1 * p1, core * 16), cs = xs + 16 * p1, g = TX_TILES / cs;
     const int bd = F->bitdepth, maxv = (1 << bd) - 1;
-    const int8_t *M1 = cta->tab8 + dct_tab8_ofs(l1), *Mt = cta->tab8 + DCT_TAB8_SIZE + dct_tab8_ofs(ln);
+    const int8_t *M1 = cta->tab8 + dct_tab8_ofs(l1), *Mt = cta->tab8 + DCT_TAB8_SIZE + dct_tab8_ofs(lc);
     const uint8_t *zz16 = (const uint8_t *)(cta->tab8 + 2 * DCT_TAB8_SIZE);
-    const FwdRound R(ln, ln - l1, bd);
+    const FwdRound R(ln, B.log2scale, bd);
     const InvRound RI(bd);
     int16_t *T = sh->tiles;
     TB_ROLL
     for (int k0 = 0; k0 < n; k0 += g) {
       const int m = min(g, n - k0);
       const tbr::TxJob<S> *G = J + k0;
-      // (1) residual -> X[k][i][j]; with `fast` the 2x2 box sums
+      // (1) residual -> X[k][i][j], the box sums
       TB_ROLL
       for (int w = l; w < (m << (2 * l1)); w += 32) {
         const int k = w >> (2 * l1), e = w & ((1 << (2 * l1)) - 1), i = e >> l1, j = e & (s1 - 1);
         const tbr::TxJob<S> &q = G[k];
-        int v = 0;
-        if (l1 == ln) v = (int)q.orig[i * q.os + j] - (int)q.pred[i * q.ps + j];
-        else
-          TB_ROLL
-          for (int t = 0; t < 4; t++) {
-            const int y = 2 * i + (t >> 1), x = 2 * j + (t & 1);
-            v += (int)q.orig[y * q.os + x] - (int)q.pred[y * q.ps + x];
-          }
-        T[k * cs + i * p1 + j] = (int16_t)v;  // modulo 2^16
+        T[k * cs + i * p1 + j] = B(i, j, [&](int y, int x) { return (int)q.orig[y * q.os + x] - (int)q.pred[y * q.ps + x]; });
       }
       sync();
       // (2) forward, first dimension: Y[k][i][j] = stage1(M[i][.] . X[k][j][.])   (i < 16, j < s1)
@@ -393,21 +370,27 @@ template <class S> struct DevBackend {
         T[k * cs + xs + (e & 15) * 24 + (e >> 4)] = (int16_t)Dequantizer(q.qp, ln)(c);
       }
       sync();
-      // (6) inverse, first dimension: X[k][j][i] = stage1(sum_t M[t][j] * rcoeff[t][i])   (j < N, i < 16; pitch 16)
+      // (6) inverse, first dimension: X[k][j][i] = stage1(sum_t M[t][j] * rcoeff[t][i])   (j < core, i < 16; pitch 16)
       TB_ROLL
-      for (int w = l; w < (m << (ln + 4)); w += 32) {
-        const int k = w >> (ln + 4), e = w & ((16 << ln) - 1), j = e >> 4, i = e & 15;
-        if ((nz >> k) & 1) T[k * cs + e] = (int16_t)InvRound::stage1(dot_rows(Mt + (j << ln), T + k * cs + xs + i * 24, 1));
+      for (int w = l; w < (m << (lc + 4)); w += 32) {
+        const int k = w >> (lc + 4), e = w & ((16 << lc) - 1), j = e >> 4, i = e & 15;
+        if ((nz >> k) & 1) T[k * cs + e] = (int16_t)InvRound::stage1(dot_rows(Mt + (j << lc), T + k * cs + xs + i * 24, 1));
       }
       sync();
-      // (7) inverse, second dimension + reconstruction: rec = clip(pred + stage2(sum_t M[t][j] * X[k][i][t])); no coefficient: rec = pred
+      // (7) inverse, second dimension + reconstruction of the rep x rep samples of core output (i, j) (i, j < core):
+      // rec = clip(pred + stage2(sum_t M[t][j] * X[k][i][t])); no coefficient: rec = pred
       TB_ROLL
-      for (int w = l; w < (m << (2 * ln)); w += 32) {
-        const int k = w >> (2 * ln), e = w & ((1 << (2 * ln)) - 1), i = e >> ln, j = e & (N - 1);
+      for (int w = l; w < (m << (2 * lc)); w += 32) {
+        const int k = w >> (2 * lc), e = w & ((1 << (2 * lc)) - 1), i = e >> lc, j = e & (core - 1);
         const tbr::TxJob<S> &q = G[k];
-        int v = (int)q.pred[i * q.ps + j];
-        if ((nz >> k) & 1) v = sat_px(v + RI.stage2(dot_rows(Mt + (j << ln), T + k * cs + i * 16, 1)), maxv);
-        q.rec[i * q.rs + j] = (S)v;
+        const bool c = (nz >> k) & 1;
+        const int r = c ? RI.stage2(dot_rows(Mt + (j << lc), T + k * cs + i * 16, 1)) : 0;
+        TB_ROLL
+        for (int t = 0; t < (1 << (2 * lr)); t++) {
+          const int y = (i << lr) + (t >> lr), x = (j << lr) + (t & ((1 << lr) - 1));
+          const int v = (int)q.pred[y * q.ps + x];
+          q.rec[y * q.rs + x] = (S)(c ? sat_px(v + r, maxv) : v);
+        }
       }
       sync();
       TB_ROLL

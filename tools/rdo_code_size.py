@@ -27,9 +27,7 @@ def main():
         elif name and re.match(r"^\s+/\*[0-9a-f]+\*/", line):
             counts[name] += 1
     rows = {"unsigned char": [], "unsigned short": []}
-    for sym, n in counts.items():
-        if "rdo_batch_kernel" not in sym:  # the translation unit also instantiates the batched kernels of tb_kernels.cuh: not part of the RD loop
-            continue
+    for sym, n in counts.items():  # the translation unit holds only the two instantiations of the RD kernel
         parts = sym.split("$")
         dem = subprocess.run(["c++filt", parts[-1] if parts[-1] else sym], capture_output=True, text=True).stdout.strip()
         dem = dem.replace("(anonymous namespace)::", "").replace("tb_rdo_tu::", "")
