@@ -185,8 +185,8 @@ int tb_interp_batch(const tb_interp_item_t *items_dev, int n, int sample_bytes, 
  * one transform block per item (the body of encode_and_reconstruct_block_*, enc/encode_block.c:1100-1338) */
 typedef struct {
   const void *orig, *pred; /* device ptrs */
-  void *rec;               /* device ptr: reconstruction out (may alias nothing) */
-  int16_t *coeffq;         /* device ptr: min(size,16)^2 quantised coefficients out (raster order) */
+  void *rec;               /* device ptr: reconstruction out (required; may alias nothing) */
+  int16_t *coeffq;         /* device ptr: min(size,16)^2 quantised coefficients out (raster order), or NULL */
   int32_t ostride, pstride, rstride;
   uint8_t size, qp, coeff_type, fast; /* coeff_type: COEFF_TYPE_* (common/global.h:103-106); fast: TB_TXFM_* flags */
 } tb_txfm_item_t;

@@ -167,9 +167,11 @@ template <class S> struct OracleBackend {
     else Orc<S>::ipred(left, top, tl, ypos + i, xpos + j, size, dst, ds, mode, F->bitdepth);
   }
   void cfl(const S *y, S *u, S *v, const S *ry, int n, int cstride, int stride) const { Orc<S>::cfl(y, u, v, ry, n, cstride, stride, 1, F->bitdepth); }
-  void tx_multi(const tbr::TxJob<S> *jobs, int n, int *bit) {  // the device runs these side by side; here one after the other
-    for (int k = 0; k < n; k++)
-      bit[k] = tx_chain(jobs[k].orig, jobs[k].os, jobs[k].pred, jobs[k].ps, jobs[k].rec, jobs[k].rs, jobs[k].cq, jobs[k].size, jobs[k].qp, jobs[k].coeff_type, jobs[k].fast);
+  void tx_multi(const tb_txfm_item_t *jobs, int n, int *bit) {  // the device runs these side by side; here one after the other
+    for (int k = 0; k < n; k++) {
+      const tb_txfm_item_t &q = jobs[k];
+      bit[k] = tx_chain((const S *)q.orig, q.ostride, (const S *)q.pred, q.pstride, (S *)q.rec, q.rstride, q.coeffq, q.size, q.qp, q.coeff_type, q.fast & TB_TXFM_FAST);
+    }
   }
   int tx_chain(const S *orig, int os, const S *pred, int ps, S *rec, int rs, int16_t *cq, int size, int qp, int coeff_type, int fast) {
     Orc<S>::residual(block, pred, orig, size, ps, os);

@@ -492,6 +492,25 @@ def test_batch_interp(tb, hbd, bd):
             assert (got[i, :bw * bh].reshape(bh, bw) == want).all(), (i, meta[i])
 
 
+def txfm_chain_in_runs(tb, items, esz, bd, hbd, recbuf, cqbuf, res, rec, cq):
+    """the batch again, its items ordered by size and `fast` flag so that the chain forms take runs of consecutive items together (up to
+    12 of 4x4/8x8, four of a larger size), every third one without coeffq: each item's result, reconstruction and levels must be those
+    of the first launch, and an item without coeffq writes no levels"""
+    n = len(items)
+    order = np.lexsort((items["fast"] & tb.TXFM_FAST, items["size"]))
+    runs = items[order].copy()
+    noq = np.arange(n) % 3 == 2
+    runs["coeffq"][noq] = 0
+    recbuf.upload(np.zeros(len(rec), sdt(hbd))); cqbuf.upload(np.zeros((n, 256), np.int16))
+    d_items = tb.DevBuf.from_array(runs); d_out = tb.DevBuf(16 * n)
+    tb.check(tb.lib.tb_txfm_chain_batch(d_items.ptr, n, esz, bd, d_out.ptr))
+    assert (d_out.download(tb.TXFM_RESULT, n) == res[order]).all()
+    assert (recbuf.download(sdt(hbd), (len(rec),)) == rec).all()
+    cq2 = cqbuf.download(np.int16, (n, 256))
+    nq = np.arange(256) < np.minimum(items["size"].astype(int), 16)[:, None] ** 2  # the levels an item writes
+    assert (cq2 == np.where(nq, cq, 0))[order[~noq]].all() and not cq2[order[noq]].any()
+
+
 @pytest.mark.parametrize("hbd,bd", BD)
 def test_batch_txfm_chain(tb, hbd, bd):
     rng = np.random.default_rng(110)
@@ -546,6 +565,7 @@ def test_batch_txfm_chain(tb, hbd, bd):
         assert int(res[i]["bits"]) == want_bits, (i, size, qp, typ, int(res[i]["bits"]), want_bits)
         ncbp += cbp
     assert 0 < ncbp < n
+    txfm_chain_in_runs(tb, items, esz, bd, hbd, recbuf, cqbuf, res, rec, cq)
 
 
 def full_scale_blocks(bd, hbd, n=128):
@@ -607,6 +627,7 @@ def test_batch_txfm_chain_full_scale(tb, hbd, bd):
         if not (int(res[i]["cbp"]) == cbp and (cq[i, :q * q] == cq0).all() and (got == want).all() and int(res[i]["ssd"]) == ssd and int(res[i]["bits"]) == bits):
             bad.append((name, size, qp, typ, fast))
     assert not bad, (len(bad), bad[:8])
+    txfm_chain_in_runs(tb, items, esz, bd, hbd, recbuf, cqbuf, res, rec, cq)
 
 
 @pytest.mark.parametrize("hbd,bd", BD)

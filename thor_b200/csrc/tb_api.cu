@@ -443,20 +443,9 @@ int tb_txfm_chain_batch(const tb_txfm_item_t *items, int n, int sample_bytes, in
   API_BEGIN();
   if (sample_bytes != 1 && sample_bytes != 2) { set_err("tb_txfm_chain_batch: sample_bytes must be 1 or 2", cudaSuccess); return TB_ERR_ARG; }
   if (n <= 0) return TB_OK;
-  size_t smem = TX_TABLE_BYTES + sizeof(TxScratch) * WARPS_PER_CTA;
-  int *meta = nullptr, *idx = nullptr;
-  CKB(cudaMallocAsync((void **)&meta, 128 * sizeof(int) + (size_t)n * sizeof(int), g.stream), "txfm scratch");
-  idx = meta + 128;
-  CKB(cudaMemsetAsync(meta, 0, 128 * sizeof(int), g.stream), "txfm scratch");
-  const int sgrid = std::min((n + 255) / 256, g.sm_count * 8);
-  const TxClassOf cls{};
-  LAUNCH((sched_hist_kernel<tb_txfm_item_t, TxClassOf>), sgrid, 256, 0, items, n, cls, meta);
-  LAUNCH(sched_scan_kernel, 1, 32, 0, meta);
-  LAUNCH((sched_scatter_kernel<tb_txfm_item_t, TxClassOf>), sgrid, 256, 0, items, n, cls, meta, idx);
-  const int grid = std::min((n + 31) / 32, g.sm_count * TX_MINBLOCKS);  // persistent: every CTA resident
-  if (sample_bytes == 1) LAUNCH(txfm_chain_kernel<uint8_t>, grid, CTA_THREADS, smem, items, n, idx, meta, bitdepth, out);
-  else LAUNCH(txfm_chain_kernel<uint16_t>, grid, CTA_THREADS, smem, items, n, idx, meta, bitdepth, out);
-  CKB(cudaFreeAsync(meta, g.stream), "txfm scratch");
+  const int grid = std::min((n + TX_CHUNK * WARPS_PER_CTA - 1) / (TX_CHUNK * WARPS_PER_CTA), g.sm_count * TX_MINBLOCKS);
+  if (sample_bytes == 1) LAUNCH(txfm_chain_kernel<uint8_t>, grid, CTA_THREADS, TX_SMEM, items, n, bitdepth, out);
+  else LAUNCH(txfm_chain_kernel<uint16_t>, grid, CTA_THREADS, TX_SMEM, items, n, bitdepth, out);
   API_END();
 }
 int tb_intra_batch(const tb_intra_item_t *items, int n, int sample_bytes, int bitdepth) {

@@ -11,6 +11,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "../../include/thor_b200.h"
 
 // TB_LDG: read-only-path load of data that no thread writes during the kernel (frames, work items).  TB_LDF: load of reconstructed
 // samples that ANOTHER CTA may have written earlier in the same kernel (wavefront RD loop, tb_rdo.cu): that translation unit maps
@@ -34,7 +35,7 @@
 namespace tb {
 
 constexpr unsigned FULL = 0xffffffffu;
-constexpr int TX_MINBLOCKS = 6;  // __launch_bounds__(128, N) of the transform-chain kernel: registers/thread <= 65536 / (128 N)
+constexpr int TX_MINBLOCKS = 5;  // __launch_bounds__(128, N) of the transform-chain kernel: registers/thread <= 65536 / (128 N); its shared memory allows 5
 constexpr int ME_MINBLOCKS = 6;  // __launch_bounds__(128, N) of the motion-search kernel: registers/thread <= 65536 / (128 N)
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
@@ -1304,11 +1305,10 @@ __device__ __forceinline__ int dct_coef(int lN, int i, int j) {  // N = 1 << lN
 // in the transform loops, which constant memory would serialise.  Layout: N=4 @0, 8 @16, 16 @80, 32 @336 (1360 entries).
 constexpr int DCT_TAB_SIZE = 1360;
 __device__ __forceinline__ int dct_tab_ofs(int lN) { return lN == 2 ? 0 : (lN == 3 ? 16 : (lN == 4 ? 80 : 336)); }
-// int8 tables, natural pitches: the 16/32-point rows are read with 128-bit loads that are uniform per quarter-warp (dot16_block)
+// int8 tables, natural pitches: the 16/32-point rows are read with 128-bit loads (dot_rows)
 constexpr int DCT_TAB8_SIZE = 16 + 64 + 16 * 16 + 32 * 32;  // 1360; every row of the 16- and 32-point tables is 16-byte aligned
 constexpr int TX_TABLE_BYTES = (DCT_TAB8_SIZE * 2 + 256 + 15) & ~15;  // int8 matrices (plain, transposed) + 16x16 zig-zag table
 __device__ __forceinline__ int dct_tab8_ofs(int lN) { return lN == 2 ? 0 : (lN == 3 ? 16 : (lN == 4 ? 80 : 336)); }
-__device__ __forceinline__ int dct_tab8_pitch(int lN) { return 1 << lN; }
 __device__ __forceinline__ void dct_tab_fill(int16_t *tab) {  // call with all threads of the CTA, then __syncthreads()
   for (int t = threadIdx.x; t < DCT_TAB_SIZE; t += blockDim.x) {
     int lN = t < 16 ? 2 : (t < 80 ? 3 : (t < 336 ? 4 : 5));
@@ -1323,50 +1323,28 @@ __device__ __forceinline__ void dct_tab8_fill(int8_t *tab8, int8_t *tab8t) {
   for (int t = threadIdx.x; t < DCT_TAB_SIZE; t += blockDim.x) {
     int lN = t < 16 ? 2 : (t < 80 ? 3 : (t < 336 ? 4 : 5));
     int e = t - dct_tab_ofs(lN), i = e >> lN, k = e & ((1 << lN) - 1);
-    int d = dct_tab8_ofs(lN) + i * dct_tab8_pitch(lN) + k;
+    int d = dct_tab8_ofs(lN) + e;
     tab8[d] = (int8_t)dct_coef(lN, i, k);
     tab8t[d] = (int8_t)dct_coef(lN, k, i);
   }
 }
-// sum += m[0..n) . v[0..n)  (m: int8 row, v: int16 row, both 4-byte aligned, n a multiple of 4): two DP2A per four terms
-__device__ __forceinline__ int dot_s8_s16(const int8_t *m, const int16_t *v, int n) {
-  int sum = 0;
-  const uint32_t *mw = (const uint32_t *)m, *vw = (const uint32_t *)v;
-  for (int k = 0; k < (n >> 2); k++) {
-    uint32_t mm = mw[k];
-    sum = __dp2a_lo((int)vw[2 * k], (int)mm, sum);
-    sum = __dp2a_hi((int)vw[2 * k + 1], (int)mm, sum);
+// m . v over 16 * nc terms (int8 matrix row, int16 vector; both 16-byte aligned): 128-bit shared loads, eight DP2A per 16 terms
+__device__ __forceinline__ int dot_rows(const int8_t *m, const int16_t *v, int nc) {
+  int t = 0;
+  TB_ROLL
+  for (int c = 0; c < nc; c++) {
+    const uint4 a = *(const uint4 *)(m + 16 * c), b0 = *(const uint4 *)(v + 16 * c), b1 = *(const uint4 *)(v + 16 * c + 8);
+    t = __dp2a_lo((int)b0.x, (int)a.x, t); t = __dp2a_hi((int)b0.y, (int)a.x, t);
+    t = __dp2a_lo((int)b0.z, (int)a.y, t); t = __dp2a_hi((int)b0.w, (int)a.y, t);
+    t = __dp2a_lo((int)b1.x, (int)a.z, t); t = __dp2a_hi((int)b1.y, (int)a.z, t);
+    t = __dp2a_lo((int)b1.z, (int)a.w, t); t = __dp2a_hi((int)b1.w, (int)a.w, t);
   }
-  return sum;
-}
-
-// acc[r][c] += A_r[0..16) . B_c[0..16): RA rows of an int8 matrix (stride sa bytes) against RB int16 vectors (stride sb elements),
-// 16 terms each.  Every operand row is fetched once with 128-bit shared loads (rows 16-byte aligned) and used RA (RB) times:
-// (RA + 2 RB) loads for 8 RA RB DP2A instead of 12 loads per 8 DP2A in the one-output-at-a-time form.
-template <int RA, int RB>
-__device__ __forceinline__ void dot16_block(const int8_t *A, int sa, const int16_t *B, int sb, int (&acc)[RA][RB]) {
-  uint4 a[RA];
-#pragma unroll
-  for (int r = 0; r < RA; r++) a[r] = *(const uint4 *)(A + r * sa);
-#pragma unroll
-  for (int c = 0; c < RB; c++) {
-    const uint4 b0 = *(const uint4 *)(B + c * sb), b1 = *(const uint4 *)(B + c * sb + 8);
-#pragma unroll
-    for (int r = 0; r < RA; r++) {
-      int t = acc[r][c];
-      t = __dp2a_lo((int)b0.x, (int)a[r].x, t); t = __dp2a_hi((int)b0.y, (int)a[r].x, t);
-      t = __dp2a_lo((int)b0.z, (int)a[r].y, t); t = __dp2a_hi((int)b0.w, (int)a[r].y, t);
-      t = __dp2a_lo((int)b1.x, (int)a[r].z, t); t = __dp2a_hi((int)b1.y, (int)a[r].z, t);
-      t = __dp2a_lo((int)b1.z, (int)a[r].w, t); t = __dp2a_hi((int)b1.w, (int)a[r].w, t);
-      acc[r][c] = t;
-    }
-  }
+  return t;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// a10-a13: the arithmetic rules of the transform chain.  Every chain form (the warp_* routines below, thread_txfm4,
-// thread_txfm8, tx_big_chain, DevBackend::tx_small / tx_mid) keeps its own data movement and takes its box sums, stage
-// rounding, scan order, quantiser and dequantiser from here.
+// a10-a13: the arithmetic rules of the transform chain.  Every chain form (the warp_* routines below, tx_small, tx_mid)
+// keeps its own data movement and takes its box sums, stage rounding, scan order, quantiser and dequantiser from here.
 // ---------------------------------------------------------------------------------------------------------------
 __constant__ uint16_t c_quant[6] = {26214, 23302, 20560, 18396, 16384, 14564};  // common/common_tables.c:72
 __constant__ uint16_t c_dequant[6] = {40, 45, 51, 57, 64, 72};                  // common/common_tables.c:73
@@ -1380,13 +1358,6 @@ __host__ __device__ constexpr int zigzag_index(int r, int c, int n) {
   const int k = (d & 1) ? (r - lo) : ((d < n ? d : n - 1) - r);
   return before + k;
 }
-// the same as a table: pos[raster position] = scan index
-template <int N> struct ZigZag {
-  uint8_t pos[N * N];
-  __host__ __device__ constexpr ZigZag() : pos() {
-    for (int p = 0; p < N * N; p++) pos[p] = (uint8_t)zigzag_index(p / N, p % N, N);
-  }
-};
 
 // Input of the forward transform, as transform_simd forms it (common/common_kernels.c:1482-1549): a size x size residual larger
 // than 32 >> fast becomes size1 x size1 box sums of scale x scale residuals, added rows outer, columns inner.  64x64 and 128x128
@@ -1588,15 +1559,14 @@ __device__ int warp_quantize_scan(const int16_t *scan, int16_t *lev, int nq, con
   return __any_sync(FULL, cbp);
 }
 // coef: compact qsize x qsize (raster) -> coefq (raster); the levels stay in sc.tmp in scan order
-__device__ int warp_quantize(const int16_t *coef, int16_t *coefq, int qp, int size, int coeff_type, TxScratch &sc, const uint8_t *zz16 = nullptr) {
+__device__ int warp_quantize(const int16_t *coef, int16_t *coefq, int qp, int size, int coeff_type, TxScratch &sc) {
   const int lane = lane_id();
   const int qsize = min(size, 16), nq = qsize * qsize, lq = ilog2(qsize);
   int16_t *scan = sc.in;  // reuse: the coefficients in scan order
-  const bool tab = zz16 != nullptr && qsize == 16;  // 16x16 scan positions from a shared-memory table instead of the closed form
-  for (int p = lane; p < nq; p += 32) scan[tab ? (int)zz16[p] : zigzag_index(p >> lq, p & (qsize - 1), qsize)] = coef[p];
+  for (int p = lane; p < nq; p += 32) scan[zigzag_index(p >> lq, p & (qsize - 1), qsize)] = coef[p];
   __syncwarp();
   const int cbp = warp_quantize_scan(scan, sc.tmp, nq, Quantizer(qp, ilog2(size), coeff_type));
-  for (int p = lane; p < nq; p += 32) coefq[p] = sc.tmp[tab ? (int)zz16[p] : zigzag_index(p >> lq, p & (qsize - 1), qsize)];
+  for (int p = lane; p < nq; p += 32) coefq[p] = sc.tmp[zigzag_index(p >> lq, p & (qsize - 1), qsize)];
   __syncwarp();
   return cbp;
 }
@@ -1640,32 +1610,6 @@ struct CoeffBitCtx {
     return bits;
   }
 };
-// one thread, N scan-ordered levels (registers when the loops unroll, local memory otherwise)
-template <int N, class Q> __device__ __forceinline__ int thread_coeff_bits(const Q &q, int size, int type) {
-  const CoeffBitCtx cx(size, type);
-  int last = -1;
-#pragma unroll(N <= 16 ? N : 1)
-  for (int p = 0; p < N; p++)
-    if (q[p]) last = p;
-  if (last < 0) return 0;
-  int bits = 0;
-  if (cx.chroma) {
-    if (last == 0 && iabs(q[0]) == 1) return 2;
-    bits = 1;
-  }
-  int S = 1, A = cx.intra && !cx.chroma, ev = -1, S_last = 1;
-#pragma unroll(N <= 16 ? N : 1)
-  for (int p = 0; p < N; p++) {
-    if (p <= last) {
-      const int c = q[p], lev = iabs(c);
-      bits += cx.pos_bits(c, S, A, p - 1 - ev);
-      if (p == last) S_last = S;
-      if (S) { if (!cx.chroma) A = lev > 3; if (!lev) S = 0; ev = p; }
-      else if (c) { S = lev > 1; ev = p; }
-    }
-  }
-  return bits + cx.tail_bits(last, N, S_last, q[last]);
-}
 // whole warp, nq (<= 256) scan-ordered levels in shared memory; every lane returns the total
 __device__ int warp_coeff_bits(const int16_t *scan, int nq, int size, int type) {
   const CoeffBitCtx cx(size, type);
@@ -1738,241 +1682,246 @@ __device__ int warp_coeff_bits(const int16_t *scan, int nq, int size, int type) 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// 4x4 transform blocks (68 % of all transform blocks in the HDB mix): ONE THREAD runs the whole chain
-// residual -> 4-point DCT x2 -> quantize -> dequantize -> inverse DCT x2 -> reconstruct -> SSD in registers.
-// Same arithmetic as the generic routines (common/transform.c:281-307, 411-465 with the 4x4 matrix :63-68,
-// enc/encode_block.c:84-160, common/common_block.c:45-83); the butterflies are exact integer refactorings of the
-// matrix products.
+// a10-a13: the transform chain (residual -> DCT -> quantiser -> dequantiser -> inverse DCT -> reconstruction) of up to 12 transform
+// blocks on one warp, for the RD loop (tb_rdo.cu) and tb_txfm_chain_batch.  Written as LOOPS over (chain, element) work items dealt
+// to the lanes: the RD loop is bound by instruction fetch, so a few KB of code that stays in the instruction cache beats unrolled or
+// register-blocked forms.  Both forms take the chain list `jobs` (which may be the job area J itself), copy it to J so that the loops
+// can index it by chain, and leave bit[k] = cbp of chain k.  Every chain writes rec and coeffq (min(size, 16)^2 levels, raster).
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void dct4_fwd(int a0, int a1, int a2, int a3, int &y0, int &y1, int &y2, int &y3) {
-  int e0 = a0 + a3, e1 = a1 + a2, o0 = a0 - a3, o1 = a1 - a2;
-  y0 = 64 * (e0 + e1); y2 = 64 * (e0 - e1); y1 = 83 * o0 + 36 * o1; y3 = 36 * o0 - 83 * o1;
-}
-__device__ __forceinline__ void dct4_inv(int x0, int x1, int x2, int x3, int &y0, int &y1, int &y2, int &y3) {
-  int e0 = 64 * (x0 + x2), e1 = 64 * (x0 - x2), o0 = 83 * x1 + 36 * x3, o1 = 36 * x1 - 83 * x3;
-  y0 = e0 + o0; y1 = e1 + o1; y2 = e1 - o1; y3 = e0 - o0;
-}
-template <class S> __device__ __forceinline__ void load_row4(const S *p, int (&v)[4]) {
-  if (sizeof(S) == 1) {
-    uint32_t w = ldw_any(p);
-#pragma unroll
-    for (int i = 0; i < 4; i++) v[i] = (int)((w >> (8 * i)) & 0xff);
-  } else {
-    uint32_t w0 = ldw_any(p), w1 = ldw_any(p + 2);
-    v[0] = (int)(w0 & 0xffff); v[1] = (int)(w0 >> 16); v[2] = (int)(w1 & 0xffff); v[3] = (int)(w1 >> 16);
-  }
-}
-template <class S> __device__ __forceinline__ void store_row4(S *p, const int (&v)[4]) {
-  if (sizeof(S) == 1 && (((uintptr_t)p) & 3) == 0) {
-    *(uint32_t *)p = (uint32_t)v[0] | ((uint32_t)v[1] << 8) | ((uint32_t)v[2] << 16) | ((uint32_t)v[3] << 24);
-  } else if (sizeof(S) == 2 && (((uintptr_t)p) & 3) == 0) {
-    ((uint32_t *)p)[0] = (uint32_t)v[0] | ((uint32_t)v[1] << 16);
-    ((uint32_t *)p)[1] = (uint32_t)v[2] | ((uint32_t)v[3] << 16);
-  } else {
-#pragma unroll
-    for (int i = 0; i < 4; i++) p[i] = (S)v[i];
+constexpr int TX_TILES = 3584;  // int16 tiles of one warp: tx_small uses 2 x 12 x 64, tx_mid up to four chains of two tiles
+
+// <= 12 chains of 16x16 to 128x128 transform blocks, all of the same size and `fast` flag: the 16- or 32-point forward transform of the s1 x s1
+// box sums of the residual (BoxSum), 16x16 coefficients, and the inverse on a core of min(N, 32) points whose every output a block larger than
+// 32x32 replicates rep x rep (common/transform.c:481-492).  One output per work item with the 16-term DP2A dot products of dot_rows.  The chains
+// of a group share every stage: four with s1 = 16 (16x16, and every size with `fast`), one with s1 = 32, in the TX_TILES int16 `tiles`.  Per
+// chain two tiles:
+//   X: box sums (s1 x s1, pitch p1) -> coefficients in scan order, quantised in place (256) -> inverse first stage, transposed (core x 16)
+//   Y: forward first stage (16 x s1, pitch p1) -> dequantised coefficients, transposed (16 x 16, pitch 24)
+// Pitches of tiles whose rows the lanes of a quarter-warp read side by side are 48 or 80 bytes: conflict-free 128-bit loads.  The quantiser's
+// level-mode walk stays warp-parallel (warp_quantize_scan), one chain after the other.  tab8: the int8 matrices, plain and transposed, and the
+// 16x16 zig-zag table (TX_TABLE_BYTES).
+template <class S>
+__device__ __noinline__ void tx_mid(const tb_txfm_item_t *jobs, int n, int *bit, const int8_t *tab8, int16_t *tiles, tb_txfm_item_t *J, int bd) {
+  const int N = jobs[0].size, ln = ilog2(N);
+  const BoxSum B(N, jobs[0].fast & TB_TXFM_FAST);
+  const int s1 = B.size1, l1 = ilog2(s1), p1 = s1 + 8, core = min(N, 32), lc = ilog2(core), lr = ln - lc;
+  const int l = lane_id();
+  __syncwarp();
+  if (l < n) J[l] = jobs[l];
+  __syncwarp();
+  const int xs = max(s1 * p1, core * 16), cs = xs + 16 * p1, g = TX_TILES / cs;
+  const int maxv = (1 << bd) - 1;
+  const int8_t *M1 = tab8 + dct_tab8_ofs(l1), *Mt = tab8 + DCT_TAB8_SIZE + dct_tab8_ofs(lc);
+  const uint8_t *zz16 = (const uint8_t *)(tab8 + 2 * DCT_TAB8_SIZE);
+  const FwdRound R(ln, B.log2scale, bd);
+  const InvRound RI(bd);
+  int16_t *T = tiles;
+  TB_ROLL
+  for (int k0 = 0; k0 < n; k0 += g) {
+    const int m = min(g, n - k0);
+    const tb_txfm_item_t *G = J + k0;
+    // (1) residual -> X[k][i][j], the box sums
+    TB_ROLL
+    for (int w = l; w < (m << (2 * l1)); w += 32) {
+      const int k = w >> (2 * l1), e = w & ((1 << (2 * l1)) - 1), i = e >> l1, j = e & (s1 - 1);
+      const tb_txfm_item_t &q = G[k];
+      const S *o = (const S *)q.orig, *p = (const S *)q.pred;
+      T[k * cs + i * p1 + j] = B(i, j, [&](int y, int x) { return (int)o[y * q.ostride + x] - (int)p[y * q.pstride + x]; });
+    }
+    __syncwarp();
+    // (2) forward, first dimension: Y[k][i][j] = stage1(M[i][.] . X[k][j][.])   (i < 16, j < s1)
+    TB_ROLL
+    for (int w = l; w < (m << (4 + l1)); w += 32) {
+      const int k = w >> (4 + l1), e = w & ((16 << l1) - 1), i = e >> l1, j = e & (s1 - 1);
+      T[k * cs + xs + i * p1 + j] = (int16_t)R.stage1(dot_rows(M1 + (i << l1), T + k * cs + j * p1, s1 >> 4));
+    }
+    __syncwarp();
+    // (3) forward, second dimension, to X[k] in scan order: X[k][zz(i, j)] = stage2(M[i][.] . Y[k][j][.])   (i, j < 16)
+    TB_ROLL
+    for (int w = l; w < (m << 8); w += 32) {
+      const int k = w >> 8, e = w & 255, i = e >> 4, j = e & 15;
+      T[k * cs + zz16[e]] = (int16_t)R.stage2(dot_rows(M1 + (i << l1), T + k * cs + xs + j * p1, s1 >> 4));
+    }
+    __syncwarp();
+    // (4) quantiser, in place, one chain after the other
+    unsigned nz = 0;
+    TB_ROLL
+    for (int k = 0; k < m; k++) {
+      const tb_txfm_item_t &q = G[k];
+      nz |= (unsigned)warp_quantize_scan(T + k * cs, T + k * cs, 256, Quantizer(q.qp, ln, q.coeff_type)) << k;
+    }
+    // (5) levels, raster, to the caller's buffer (reference layout) and, dequantised, transposed to Y[k][j][i] = rcoeff[i][j] (pitch 24)
+    TB_ROLL
+    for (int w = l; w < (m << 8); w += 32) {
+      const int k = w >> 8, e = w & 255;
+      const tb_txfm_item_t &q = G[k];
+      const int c = T[k * cs + zz16[e]];
+      q.coeffq[e] = (int16_t)c;
+      T[k * cs + xs + (e & 15) * 24 + (e >> 4)] = (int16_t)Dequantizer(q.qp, ln)(c);
+    }
+    __syncwarp();
+    // (6) inverse, first dimension: X[k][j][i] = stage1(sum_t M[t][j] * rcoeff[t][i])   (j < core, i < 16; pitch 16)
+    TB_ROLL
+    for (int w = l; w < (m << (lc + 4)); w += 32) {
+      const int k = w >> (lc + 4), e = w & ((16 << lc) - 1), j = e >> 4, i = e & 15;
+      if ((nz >> k) & 1) T[k * cs + e] = (int16_t)InvRound::stage1(dot_rows(Mt + (j << lc), T + k * cs + xs + i * 24, 1));
+    }
+    __syncwarp();
+    // (7) inverse, second dimension + reconstruction of the rep x rep samples of core output (i, j) (i, j < core):
+    // rec = clip(pred + stage2(sum_t M[t][j] * X[k][i][t])); no coefficient: rec = pred
+    TB_ROLL
+    for (int w = l; w < (m << (2 * lc)); w += 32) {
+      const int k = w >> (2 * lc), e = w & ((1 << (2 * lc)) - 1), i = e >> lc, j = e & (core - 1);
+      const tb_txfm_item_t &q = G[k];
+      const S *p = (const S *)q.pred;
+      S *rec = (S *)q.rec;
+      const bool c = (nz >> k) & 1;
+      const int r = c ? RI.stage2(dot_rows(Mt + (j << lc), T + k * cs + i * 16, 1)) : 0;
+      TB_ROLL
+      for (int t = 0; t < (1 << (2 * lr)); t++) {
+        const int y = (i << lr) + (t >> lr), x = (j << lr) + (t & ((1 << lr) - 1));
+        const int v = (int)p[y * q.pstride + x];
+        rec[y * q.rstride + x] = (S)(c ? sat_px(v + r, maxv) : v);
+      }
+    }
+    __syncwarp();
+    TB_ROLL
+    for (int k = 0; k < m; k++) bit[k0 + k] = (nz >> k) & 1;
   }
 }
 
-// returns cbp; ssd out
+// <= 12 chains of 4x4 / 8x8 transform blocks (the arithmetic of common/transform.c:245-308, 411-494, enc/encode_block.c:84-171,
+// common/common_block.c:45-83), all of them together on the warp.  Tiles of 64 int16 per chain in `tiles`; the quantiser's level-mode walk is
+// sequential: one lane per chain.  tab16: the int16 matrices (dct_tab_fill).
 template <class S>
-__device__ int thread_txfm4(const S *orig, int os, const S *pred, int ps, S *rec, int rs, int16_t *coeffq_out, int qp, int coeff_type, int bitdepth,
-                            uint64_t &ssd_out, int want_bits, int &bits_out) {
-  constexpr ZigZag<4> ZZ;
-  const int maxv = (1 << bitdepth) - 1;
-  int o[16], p[16], t[16], c[16];
-#pragma unroll
-  for (int r = 0; r < 4; r++) {
-    int a[4], b[4];
-    load_row4<S>(orig + r * os, a);
-    load_row4<S>(pred + r * ps, b);
-#pragma unroll
-    for (int k = 0; k < 4; k++) { o[r * 4 + k] = a[k]; p[r * 4 + k] = b[k]; }
+__device__ __noinline__ void tx_small(const tb_txfm_item_t *jobs, int n, int *bit, const int16_t *tab16, int16_t *tiles, tb_txfm_item_t *J, int bd) {
+  const int l = lane_id();
+  int16_t *A = tiles, *B = tiles + 768;  // 12 tiles of 64 each
+  __syncwarp();
+  if (l < n) J[l] = jobs[l];
+  __syncwarp();
+  const int maxv = (1 << bd) - 1;
+  // (1) residual -> A[k][i * N + j]
+  TB_ROLL
+  for (int w = l; w < n * 64; w += 32) {
+    const int k = w >> 6, e = w & 63;
+    const tb_txfm_item_t &q = J[k];
+    const int N = q.size, ln = N == 8 ? 3 : 2;
+    if (e < N * N) {
+      const int i = e >> ln, j = e & (N - 1);
+      A[w] = (int16_t)((int)((const S *)q.orig)[i * q.ostride + j] - (int)((const S *)q.pred)[i * q.pstride + j]);
+    }
   }
-  // forward, 1st dimension: t[i][j] = stage1(sum_k M[i][k] * res[j][k])
-  const FwdRound R(2, 0, bitdepth);
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    int y0, y1, y2, y3;
-    dct4_fwd(o[j * 4] - p[j * 4], o[j * 4 + 1] - p[j * 4 + 1], o[j * 4 + 2] - p[j * 4 + 2], o[j * 4 + 3] - p[j * 4 + 3], y0, y1, y2, y3);
-    t[0 * 4 + j] = R.stage1(y0); t[1 * 4 + j] = R.stage1(y1); t[2 * 4 + j] = R.stage1(y2); t[3 * 4 + j] = R.stage1(y3);
+  __syncwarp();
+  // (2) forward, first dimension: B[k][i][j] = stage1(sum_t M[i][t] * A[k][j][t])
+  TB_ROLL
+  for (int w = l; w < n * 64; w += 32) {
+    const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
+    if (e < N * N) {
+      const int i = e >> ln, j = e & (N - 1);
+      const int16_t *M = tab16 + (N == 8 ? 16 : 0) + (i << ln), *a = A + (k << 6) + (j << ln);
+      int sum = 0;
+      TB_ROLL
+      for (int t = 0; t < N; t++) sum += (int)M[t] * (int)a[t];
+      B[w] = (int16_t)FwdRound(ln, 0, bd).stage1(sum);
+    }
   }
-  // 2nd dimension: coef[i][j] = stage2(sum_k M[i][k] * t[j][k]), stored straight into scan order
-  int sc[16];
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    int y0, y1, y2, y3;
-    dct4_fwd(t[j * 4], t[j * 4 + 1], t[j * 4 + 2], t[j * 4 + 3], y0, y1, y2, y3);
-    sc[ZZ.pos[0 * 4 + j]] = R.stage2(y0); sc[ZZ.pos[1 * 4 + j]] = R.stage2(y1);
-    sc[ZZ.pos[2 * 4 + j]] = R.stage2(y2); sc[ZZ.pos[3 * 4 + j]] = R.stage2(y3);
+  __syncwarp();
+  // (3) forward, second dimension: A[k][i][j] = stage2(sum_t M[i][t] * B[k][j][t])   (coefficients, raster)
+  TB_ROLL
+  for (int w = l; w < n * 64; w += 32) {
+    const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
+    int v = 0;
+    if (e < N * N) {
+      const int i = e >> ln, j = e & (N - 1);
+      const int16_t *M = tab16 + (N == 8 ? 16 : 0) + (i << ln), *b = B + (k << 6) + (j << ln);
+      int sum = 0;
+      TB_ROLL
+      for (int t = 0; t < N; t++) sum += (int)M[t] * (int)b[t];
+      v = FwdRound(ln, 0, bd).stage2(sum);
+    }
+    if (e < N * N) A[w] = (int16_t)v;  // A was consumed by (2)
   }
-  const Quantizer Q(qp, 2, coeff_type);
-  int last = -1;
-#pragma unroll
-  for (int pos = 0; pos < 16; pos++)
-    if (Q.last_nz(sc[pos])) last = pos;
-  int mode = 1, cbp = 0, q[16];
-#pragma unroll
-  for (int pos = 0; pos < 16; pos++) {
-    int lev = 0;
-    if (pos <= last) {
-      lev = Q.level(sc[pos], mode);
+  __syncwarp();
+  // (4) zig-zag scan order -> B[k][pos]
+  TB_ROLL
+  for (int w = l; w < n * 64; w += 32) {
+    const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
+    if (e < N * N) B[(k << 6) + zigzag_index(e >> ln, e & (N - 1), N)] = A[w];
+  }
+  __syncwarp();
+  // (5) quantiser (sequential level-mode walk), lane k on chain k: levels in scan order -> B[k][pos] in place; cbp
+  int cbp = 0;
+  if (l < n) {
+    const tb_txfm_item_t &q = J[l];
+    const int N = q.size, nq = N * N;
+    const Quantizer Q(q.qp, N == 8 ? 3 : 2, q.coeff_type);
+    int16_t *sc_ = B + (l << 6);
+    bool nz = false;
+    int pos = nq - 1;
+    while (!nz && pos >= 0) nz = Q.last_nz(sc_[pos--]);
+    const int last_pos = nz ? pos + 1 : pos;
+    int level_mode = 1;
+    TB_ROLL
+    for (pos = 0; pos <= last_pos; pos++) {
+      const int c = sc_[pos], lev = Q.level(c, level_mode);
+      sc_[pos] = (int16_t)(c < 0 ? -lev : lev);
       cbp |= lev != 0;
-      mode = Quantizer::next_mode(mode, lev);
+      level_mode = Quantizer::next_mode(level_mode, lev);
     }
-    q[pos] = sc[pos] < 0 ? -lev : lev;
+    TB_ROLL
+    for (pos = last_pos + 1; pos < nq; pos++) sc_[pos] = 0;
   }
-  if (coeffq_out) {
-#pragma unroll
-    for (int r = 0; r < 16; r++) coeffq_out[r] = (int16_t)q[ZZ.pos[r]];
-  }
-  bits_out = (want_bits && cbp) ? thread_coeff_bits<16>(q, 4, coeff_type) : 0;
-  uint64_t ssd = 0;
-  if (cbp) {
-    const Dequantizer D(qp, 2);
-#pragma unroll
-    for (int r = 0; r < 16; r++) c[r] = D(q[ZZ.pos[r]]);
-    // inverse, 1st dimension: t[i][j] = stage1(sum_k M[k][j] * c[k][i])
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      int y0, y1, y2, y3;
-      dct4_inv(c[0 * 4 + i], c[1 * 4 + i], c[2 * 4 + i], c[3 * 4 + i], y0, y1, y2, y3);
-      t[i * 4 + 0] = InvRound::stage1(y0); t[i * 4 + 1] = InvRound::stage1(y1);
-      t[i * 4 + 2] = InvRound::stage1(y2); t[i * 4 + 3] = InvRound::stage1(y3);
+  __syncwarp();
+  const unsigned nzmask = __ballot_sync(FULL, cbp != 0);
+  // (6) quantised coefficients, raster: to the caller's buffer (reference layout) and, dequantised, to A[k] (dequantize(), common/common_block.c:45)
+  TB_ROLL
+  for (int w = l; w < n * 64; w += 32) {
+    const int k = w >> 6, e = w & 63;
+    const tb_txfm_item_t &q = J[k];
+    const int N = q.size, ln = N == 8 ? 3 : 2;
+    if (e < N * N) {
+      const int c = B[(k << 6) + zigzag_index(e >> ln, e & (N - 1), N)];
+      q.coeffq[e] = (int16_t)c;
+      A[w] = (int16_t)Dequantizer(q.qp, ln)(c);
     }
-    // 2nd dimension + reconstruction: out[i][j] = stage2(sum_k M[k][j] * t[k][i])
-    const InvRound RI(bitdepth);
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      int y[4];
-      dct4_inv(t[0 * 4 + i], t[1 * 4 + i], t[2 * 4 + i], t[3 * 4 + i], y[0], y[1], y[2], y[3]);
-      int v[4];
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        int r = RI.stage2(y[j]);
-        v[j] = sat_px(r + p[i * 4 + j], maxv);
-        int d = o[i * 4 + j] - v[j];
-        ssd += (uint32_t)(d * d);
+  }
+  __syncwarp();
+  // (7) inverse, first dimension: B[k][i][j] = stage1(sum_t M[t][j] * A[k][t][i])
+  TB_ROLL
+  for (int w = l; w < n * 64; w += 32) {
+    const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
+    if (e < N * N && ((nzmask >> k) & 1)) {
+      const int i = e >> ln, j = e & (N - 1);
+      const int16_t *M = tab16 + (N == 8 ? 16 : 0), *a = A + (k << 6);
+      int o = 0;
+      TB_ROLL
+      for (int t = 0; t < N; t++) o += (int)M[(t << ln) + j] * (int)a[(t << ln) + i];
+      B[w] = (int16_t)InvRound::stage1(o);
+    }
+  }
+  __syncwarp();
+  // (8) inverse, second dimension + reconstruction: rec = clip(pred + stage2(sum_t M[t][j] * B[k][t][i])); no coefficient: rec = pred
+  TB_ROLL
+  for (int w = l; w < n * 64; w += 32) {
+    const int k = w >> 6, e = w & 63;
+    const tb_txfm_item_t &q = J[k];
+    const int N = q.size, ln = N == 8 ? 3 : 2;
+    if (e < N * N) {
+      const int i = e >> ln, j = e & (N - 1);
+      int v = (int)((const S *)q.pred)[i * q.pstride + j];
+      if ((nzmask >> k) & 1) {
+        const int16_t *M = tab16 + (N == 8 ? 16 : 0), *b = B + (k << 6);
+        int o = 0;
+        TB_ROLL
+        for (int t = 0; t < N; t++) o += (int)M[(t << ln) + j] * (int)b[(t << ln) + i];
+        v = sat_px(v + InvRound(bd).stage2(o), maxv);
       }
-      if (rec) store_row4<S>(rec + i * rs, v);
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      int v[4];
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        v[j] = p[i * 4 + j];
-        int d = o[i * 4 + j] - v[j];
-        ssd += (uint32_t)(d * d);
-      }
-      if (rec) store_row4<S>(rec + i * rs, v);
+      ((S *)q.rec)[i * q.rstride + j] = (S)v;
     }
   }
-  ssd_out = ssd;
-  return cbp;
-}
-
-// 8x8 transform blocks: also one THREAD per block.  The 64-entry work arrays live in local memory, which the hardware
-// interleaves per thread, so the lock-step (uniform-index) accesses of a warp coalesce into L1 lines; the DCT matrix is
-// read from the shared-memory table with a warp-uniform index (broadcast).  Same arithmetic as warp_fwd_transform /
-// warp_quantize / warp_dequantize / warp_inv_transform.
-__constant__ ZigZag<8> c_zz8;  // not const: a const table is folded into the code, which costs thread_txfm8 spills
-// eight-term dot product of an int8 matrix row (two words) with eight int16 values (four words): four DP2A
-__device__ __forceinline__ int dot8(uint2 m, uint4 v, int acc) {
-  acc = __dp2a_lo((int)v.x, (int)m.x, acc);
-  acc = __dp2a_hi((int)v.y, (int)m.x, acc);
-  acc = __dp2a_lo((int)v.z, (int)m.y, acc);
-  return __dp2a_hi((int)v.w, (int)m.y, acc);
-}
-template <class S>
-__device__ int thread_txfm8(const S *orig, int os, const S *pred, int ps, S *rec, int rs, int16_t *coeffq_out, int qp, int coeff_type, int bitdepth,
-                            const int8_t *tab8, const int8_t *tab8t, uint64_t &ssd_out, int want_bits, int &bits_out) {
-  const uint2 *M = (const uint2 *)(tab8 + dct_tab8_ofs(3)), *Mt = (const uint2 *)(tab8t + dct_tab8_ofs(3));  // rows of 8 int8, warp-uniform index
-  const int maxv = (1 << bitdepth) - 1;
-  alignas(16) int16_t a[64], b[64];  // 16-byte rows: each row is one 128-bit local load in the matrix phases
-  for (int r = 0; r < 8; r++) {
-    int o0[4], o1[4], p0[4], p1[4];
-    load_row4<S>(orig + r * os, o0); load_row4<S>(orig + r * os + 4, o1);
-    load_row4<S>(pred + r * ps, p0); load_row4<S>(pred + r * ps + 4, p1);
-    *(uint4 *)&a[r * 8] = make_uint4(((uint32_t)(o0[0] - p0[0]) & 0xffffu) | ((uint32_t)(o0[1] - p0[1]) << 16), ((uint32_t)(o0[2] - p0[2]) & 0xffffu) | ((uint32_t)(o0[3] - p0[3]) << 16),
-                                     ((uint32_t)(o1[0] - p1[0]) & 0xffffu) | ((uint32_t)(o1[1] - p1[1]) << 16), ((uint32_t)(o1[2] - p1[2]) & 0xffffu) | ((uint32_t)(o1[3] - p1[3]) << 16));
-  }
-  // forward: b[i][j] = stage1(M[i] . res[j]), then a[scan(i, j)] = stage2(M[i] . b[j])
-  const FwdRound R(3, 0, bitdepth);
-  for (int j = 0; j < 8; j++) {
-    const uint4 v = *(const uint4 *)&a[j * 8];
-#pragma unroll
-    for (int i = 0; i < 8; i++) b[i * 8 + j] = (int16_t)R.stage1(dot8(M[i], v, 0));
-  }
-  for (int j = 0; j < 8; j++) {
-    const uint4 v = *(const uint4 *)&b[j * 8];
-#pragma unroll
-    for (int i = 0; i < 8; i++) a[c_zz8.pos[i * 8 + j]] = (int16_t)R.stage2(dot8(M[i], v, 0));  // scan order
-  }
-  const Quantizer Q(qp, 3, coeff_type);
-  int last = -1;
-  for (int pos = 0; pos < 64; pos++)
-    if (Q.last_nz(a[pos])) last = pos;
-  int mode = 1, cbp = 0;
-  for (int pos = 0; pos < 64; pos++) {
-    int lev = 0, cc = a[pos];
-    if (pos <= last) {
-      lev = Q.level(cc, mode);
-      cbp |= lev != 0;
-      mode = Quantizer::next_mode(mode, lev);
-    }
-    b[pos] = (int16_t)(cc < 0 ? -lev : lev);  // quantised, scan order
-  }
-  if (coeffq_out)
-    for (int p = 0; p < 64; p++) coeffq_out[p] = b[c_zz8.pos[p]];
-  bits_out = (want_bits && cbp) ? thread_coeff_bits<64>(b, 8, coeff_type) : 0;
-  uint64_t ssd = 0;
-  if (cbp) {
-    // de-quantise into the TRANSPOSED block a[i][k] = rcoeff[k][i], so that both inverse stages are row . row products
-    const Dequantizer D(qp, 3);
-    for (int k = 0; k < 8; k++)
-#pragma unroll
-      for (int i = 0; i < 8; i++) a[i * 8 + k] = (int16_t)D(b[c_zz8.pos[k * 8 + i]]);
-    // inverse 1st dimension: T[i][j] = stage1(sum_k M[k][j] * rcoeff[k][i]), stored transposed: b[j][i]
-    for (int i = 0; i < 8; i++) {
-      const uint4 v = *(const uint4 *)&a[i * 8];
-#pragma unroll
-      for (int j = 0; j < 8; j++) b[j * 8 + i] = (int16_t)InvRound::stage1(dot8(Mt[j], v, 0));
-    }
-    // 2nd dimension + reconstruction: out[i][j] = stage2(sum_k M[k][j] * T[k][i]) = stage2(Mt[j] . b[i])
-    const InvRound RI(bitdepth);
-    for (int i = 0; i < 8; i++) {
-      const uint4 v = *(const uint4 *)&b[i * 8];
-#pragma unroll
-      for (int h2 = 0; h2 < 2; h2++) {
-        int pv[4], ov[4], o4[4];
-        load_row4<S>(pred + i * ps + 4 * h2, pv);
-        load_row4<S>(orig + i * os + 4 * h2, ov);
-#pragma unroll
-        for (int t = 0; t < 4; t++) {
-          int r = RI.stage2(dot8(Mt[4 * h2 + t], v, 0));
-          o4[t] = sat_px(r + pv[t], maxv);
-          int d = ov[t] - o4[t];
-          ssd += (uint32_t)(d * d);
-        }
-        if (rec) store_row4<S>(rec + i * rs + 4 * h2, o4);
-      }
-    }
-  } else {
-    for (int i = 0; i < 8; i++)
-#pragma unroll
-      for (int h2 = 0; h2 < 2; h2++) {
-        int pv[4], ov[4];
-        load_row4<S>(pred + i * ps + 4 * h2, pv);
-        load_row4<S>(orig + i * os + 4 * h2, ov);
-        if (rec) store_row4<S>(rec + i * rs + 4 * h2, pv);
-#pragma unroll
-        for (int t = 0; t < 4; t++) { int d = ov[t] - pv[t]; ssd += (uint32_t)(d * d); }
-      }
-  }
-  ssd_out = ssd;
-  return cbp;
+  __syncwarp();
+  for (int k = 0; k < n; k++) bit[k] = (nzmask >> k) & 1;
 }
 
 // a13: dequantize.  common/common_block.c:45-73 (no weight matrix).  compact in, compact out (pitch qsize)

@@ -73,7 +73,7 @@ __device__ __forceinline__ int me_class(int w, int h, int speed) {
 }
 // meta layout (ints): [0,32) histogram, [32,64) first list position of each class, [64,96) fill cursors, 96 = number of team
 // items, 97 = team cursor, 98 = warp cursor, 99 = number of listed items, 100 = group cursor.  A class functor returns the
-// class (0..31; >= 16: searched/transformed by the whole CTA) of an item, or -1 when the item is not listed.
+// class (0..31; >= 16: searched by the whole CTA) of an item, or -1 when the item is not listed.
 struct MeClassOf {
   int speed, quad;  // quad: 8-bit samples and speed 0 -> blocks of <= 64 samples are listed too (class 1) and searched four per warp
   __device__ __forceinline__ int operator()(const tb_me_item_t &q) const {
@@ -84,9 +84,6 @@ struct MeClassOf {
       return 1;
     return -1;  // the others are drawn from the caller's array in its own order
   }
-};
-struct TxClassOf {  // transform blocks > 8x8 are listed (one warp each, the CTA for >= 64x64); 4x4 / 8x8 run one per thread
-  __device__ __forceinline__ int operator()(const tb_txfm_item_t &q) const { return q.size >= 64 ? 16 + ilog2(q.size) : (q.size > 8 ? ilog2(q.size) : -1); }
 };
 template <class Item, class F> __global__ void sched_hist_kernel(const Item *items, int n, F f, int *meta) {
   __shared__ int h[32];
@@ -295,352 +292,97 @@ template <class S> __global__ void block_avg_kernel(S *p, int sp, const S *r0, i
 }
 
 // ---- a10-a13 + a3 ----------------------------------------------------------------------------------------------
-struct alignas(16) TxShared {
-  TxScratch sc;
+// The chains of tb_txfm_chain_batch run on the RD loop's forms.  Each warp takes chunks of TX_CHUNK consecutive items (grid-stride)
+// and runs every run of consecutive items that one call takes together, in the caller's order: 4x4 and 8x8 items go to tx_small,
+// items of the same larger size and `fast` flag to tx_mid, up to four (its largest group).  Then the SSD and, with TB_TXFM_BITS,
+// the bit count of each item, as the RD loop's DevBackend::ssd / coeff_bits compute them.  An item without coeffq leaves its levels
+// in the warp's `lev`: 12 chains of <= 8x8 or four larger ones fit.
+constexpr int TX_CHUNK = 12;
+struct TxWarp {
+  alignas(16) int16_t tiles[TX_TILES];
+  alignas(16) int16_t lev[1024];
+  tb_txfm_item_t jobs[TX_CHUNK];
 };
-
-// residual on the fly -> forward -> quantise -> de-quantise -> inverse -> reconstruct + SSD.
-// One transform block > 8x8 handled by a team of TW warps (TW == 1: a warp; TW == WARPS_PER_CTA: the CTA, for 64x64 and
-// 128x128 whose box-sum load and replicated output are per-sample passes over up to 16384 samples).
-template <class S, int TW>
-__device__ __noinline__ void tx_big_chain(const tb_txfm_item_t &q, int bitdepth, TxScratch &sc, int16_t *rt, const int8_t *tab8, const int8_t *tab8t, unsigned long long *red,
-                                          int *bc, tb_txfm_result_t *res) {
-  const uint8_t *zz16 = (const uint8_t *)(tab8 + 2 * DCT_TAB8_SIZE);  // 16x16 zig-zag table behind the two matrix tables
-  constexpr int PI = 40;  // int16 pitch of the scratch tiles: 80-byte rows (16-byte aligned; eight consecutive rows cover all 32 banks with 128-bit loads)
-  constexpr int NT = 32 * TW;
-  const int tid = TW == 1 ? lane_id() : (int)threadIdx.x, lane = lane_id(), maxv = (1 << bitdepth) - 1;
-  auto sync = [&]() { if (TW == 1) __syncwarp(); else __syncthreads(); };
-  const S *orig = (const S *)q.orig, *pred = (const S *)q.pred;
-  S *rec = (S *)q.rec;
-  const int size = q.size;
-  const int fast = q.fast & 1, want_bits = q.fast & 2;  // flags byte: TB_TXFM_FAST | TB_TXFM_BITS
-  const BoxSum B(size, fast);
-  const int size1 = B.size1, scale = B.scale();
-  const int l1 = ilog2(size1), qsize = min(size, 16), lq = ilog2(qsize);
-  const int8_t *M1 = tab8 + dct_tab8_ofs(l1);
-  const int mp1 = dct_tab8_pitch(l1);
-  // residual (enc/encode_block.c:162-171) fused with the box-sum load of the forward transform (BoxSum), rows of four samples per load
-  if (scale == 1) {
-    for (int p = tid; p < (size1 * size1) >> 2; p += NT) {  // four samples per thread and step
-      int i = p >> (l1 - 2), j = (p & ((size1 >> 2) - 1)) << 2;
-      int a[4], b[4];
-      load_row4<S>(orig + i * q.ostride + j, a);
-      load_row4<S>(pred + i * q.pstride + j, b);
-      *(uint2 *)&sc.in[i * PI + j] = make_uint2(((uint32_t)(a[0] - b[0]) & 0xffffu) | ((uint32_t)(a[1] - b[1]) << 16), ((uint32_t)(a[2] - b[2]) & 0xffffu) | ((uint32_t)(a[3] - b[3]) << 16));
-    }
-  } else if (scale == 2) {  // 64x64 or 32x32 with `fast`
-    for (int p = tid; p < (size1 * size1) >> 1; p += NT) {  // two outputs (four source columns) per thread and step
-      int i = p >> (l1 - 1), j = (p & ((size1 >> 1) - 1)) << 1, s0 = 0, s1 = 0;
-      for (int m = 0; m < 2; m++) {
-        int a[4], b[4];
-        load_row4<S>(orig + (i * 2 + m) * q.ostride + j * 2, a);
-        load_row4<S>(pred + (i * 2 + m) * q.pstride + j * 2, b);
-        s0 = B.add(B.add(s0, a[0] - b[0]), a[1] - b[1]);
-        s1 = B.add(B.add(s1, a[2] - b[2]), a[3] - b[3]);
-      }
-      sc.in[i * PI + j] = (int16_t)s0;
-      sc.in[i * PI + j + 1] = (int16_t)s1;
-    }
-  } else {  // 128x128, or 64x64 with `fast`
-    for (int p = tid; p < size1 * size1; p += NT) {
-      int i = p >> l1, j = p & (size1 - 1), sum = 0;
-      for (int m = 0; m < scale; m++)
-        for (int n = 0; n < scale; n += 4) {
-          int a[4], b[4];
-          load_row4<S>(orig + (i * scale + m) * q.ostride + j * scale + n, a);
-          load_row4<S>(pred + (i * scale + m) * q.pstride + j * scale + n, b);
-#pragma unroll
-          for (int t = 0; t < 4; t++) sum = B.add(sum, a[t] - b[t]);
-        }
-      sc.in[i * PI + j] = (int16_t)sum;
-    }
-  }
-  sync();
-  // The transform phases run on one warp (the first warp of a team: they are a small part of a 64x64/128x128 chain).  Lane
-  // (ia = lane >> 3, jb = lane & 7) owns the outputs {4 ia .. 4 ia + 3} x {jb, jb + 8, ..}: the matrix rows are uniform per
-  // quarter-warp (broadcast) and the vectors of a quarter-warp are eight consecutive 80-byte rows (conflict-free).
-  const bool dct_warp = TW == 1 || threadIdx.x < 32;
-  const int ia = lane >> 3, jb = lane & 7;
-  {
-    const FwdRound R(ilog2(size), ilog2(scale), bitdepth);
-    // tmp[i][j] = stage1(M[i][.] . in[j][.])   (i < 16, j < size1)
-    if (dct_warp) {
-      if (size1 == 16) {
-        int acc[4][2] = {};
-        dot16_block<4, 2>(M1 + 4 * ia * mp1, mp1, sc.in + jb * PI, 8 * PI, acc);
-#pragma unroll
-        for (int r = 0; r < 4; r++)
-#pragma unroll
-          for (int c = 0; c < 2; c++) sc.tmp[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)R.stage1(acc[r][c]);
-      } else {
-        int acc[4][4] = {};
-        dot16_block<4, 4>(M1 + 4 * ia * mp1, mp1, sc.in + jb * PI, 8 * PI, acc);
-        dot16_block<4, 4>(M1 + 4 * ia * mp1 + 16, mp1, sc.in + jb * PI + 16, 8 * PI, acc);
-#pragma unroll
-        for (int r = 0; r < 4; r++)
-#pragma unroll
-          for (int c = 0; c < 4; c++) sc.tmp[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)R.stage1(acc[r][c]);
-      }
-    }
-    sync();
-    // coef[i][j] = stage2(M[i][.] . tmp[j][.])  (i, j < 16)
-    if (dct_warp) {
-      int acc[4][2] = {};
-      dot16_block<4, 2>(M1 + 4 * ia * mp1, mp1, sc.tmp + jb * PI, 8 * PI, acc);
-      if (size1 == 32) dot16_block<4, 2>(M1 + 4 * ia * mp1 + 16, mp1, sc.tmp + jb * PI + 16, 8 * PI, acc);
-#pragma unroll
-      for (int r = 0; r < 4; r++)
-#pragma unroll
-        for (int c = 0; c < 2; c++) sc.rc[(4 * ia + r) * 16 + jb + 8 * c] = (int16_t)R.stage2(acc[r][c]);
-    }
-    sync();
-  }
-  int cbp;
-  if (TW == 1) cbp = warp_quantize(sc.rc, sc.cq, q.qp, size, q.coeff_type, sc, zz16);
-  else {
-    if (threadIdx.x < 32) {
-      int c = warp_quantize(sc.rc, sc.cq, q.qp, size, q.coeff_type, sc, zz16);
-      if (lane == 0) *bc = c;
-    }
-    __syncthreads();
-    cbp = *bc;
-  }
-  if (q.coeffq)
-    for (int p = tid; p < qsize * qsize; p += NT) q.coeffq[p] = sc.cq[p];
-  int bits = 0;
-  if (want_bits && cbp && dct_warp) bits = warp_coeff_bits(sc.tmp, qsize * qsize, size, q.coeff_type);  // sc.tmp: the levels in scan order (warp_quantize)
-  uint64_t ssd = 0;
-  if (cbp) {
-    // de-quantise (common/common_block.c:45-73) straight into the TRANSPOSED tile in[i][k] = rcoeff[k][i], so that the
-    // inverse transform's sums over k read contiguous int16 pairs
-    {
-      const Dequantizer D(q.qp, ilog2(size));
-      for (int p = tid; p < qsize * qsize; p += NT) {
-        int k = p >> lq, i = p & (qsize - 1);
-        sc.in[i * PI + k] = (int16_t)D(sc.cq[p]);
-      }
-      sync();
-    }
-    // inverse transform with the reconstruction (common/common_block.c:75-83) and SSD fused into its output stage
-    const int core = min(size, 32), rep = size / core, lc = ilog2(core);
-    const InvRound RI(bitdepth);
-    const int8_t *Mt = tab8t + dct_tab8_ofs(lc);
-    const int mpc = dct_tab8_pitch(lc);
-    // T[i][j] = stage1(sum_k M[k][j] * rcoeff[k][i]), stored transposed: tmp2[j][i]   (i < 16, j < core)
-    int16_t *tmp2 = sc.in + 16 * PI;  // rows 16.. of the `in` tile are free here (rcoeff^T uses rows 0..15)
-    if (dct_warp) {
-      if (core == 16) {
-        int acc[4][2] = {};
-        dot16_block<4, 2>(Mt + 4 * ia * mpc, mpc, sc.in + jb * PI, 8 * PI, acc);
-#pragma unroll
-        for (int r = 0; r < 4; r++)
-#pragma unroll
-          for (int c = 0; c < 2; c++) tmp2[(4 * ia + r) * PI + jb + 8 * c] = (int16_t)InvRound::stage1(acc[r][c]);
-      } else {
-#pragma unroll
-        for (int half = 0; half < 2; half++) {
-          int acc[4][2] = {};
-          dot16_block<4, 2>(Mt + (16 * half + 4 * ia) * mpc, mpc, sc.in + jb * PI, 8 * PI, acc);
-#pragma unroll
-          for (int r = 0; r < 4; r++)
-#pragma unroll
-            for (int c = 0; c < 2; c++) tmp2[(16 * half + 4 * ia + r) * PI + jb + 8 * c] = (int16_t)InvRound::stage1(acc[r][c]);
-        }
-      }
-    }
-    sync();
-    // out[i][j] = stage2(sum_k M[k][j] * T[k][i]) = stage2(Mt[j][.] . tmp2[i][.])   (i, j < core); lane (jg = lane >> 3,
-    // il = lane & 7) owns columns 4 jg .. 4 jg + 3 (+16 in a second pass for core 32) of rows il, il + 8, ..
-    if (rep == 1) {
-      if (dct_warp) {
-        for (int jg = ia; jg < (core >> 2); jg += 4) {
-          for (int i0 = jb; i0 < core; i0 += 16) {
-            int acc[4][2] = {};
-            dot16_block<4, 2>(Mt + 4 * jg * mpc, mpc, tmp2 + i0 * PI, 8 * PI, acc);
-#pragma unroll
-            for (int c = 0; c < 2; c++) {
-              const int i = i0 + 8 * c, j = 4 * jg;
-              int pv[4], ov[4], v[4];
-              load_row4<S>(pred + i * q.pstride + j, pv);
-              load_row4<S>(orig + i * q.ostride + j, ov);
-#pragma unroll
-              for (int t = 0; t < 4; t++) {
-                int r = RI.stage2(acc[t][c]);
-                v[t] = sat_px(r + pv[t], maxv);
-                int d = ov[t] - v[t];
-                ssd += (uint64_t)(uint32_t)(d * d);
-              }
-              if (rec) store_row4<S>(rec + i * q.rstride + j, v);
-            }
-          }
-        }
-      }
-    } else if (TW > 1 && (rep == 2 || rep == 4)) {
-      // the core x core residual goes to a second tile, then one per-sample pass replicates it (common/transform.c:481-492)
-      if (dct_warp) {
-        for (int jg = ia; jg < (core >> 2); jg += 4) {
-          for (int i0 = jb; i0 < core; i0 += 16) {
-            int acc[4][2] = {};
-            dot16_block<4, 2>(Mt + 4 * jg * mpc, mpc, tmp2 + i0 * PI, 8 * PI, acc);
-#pragma unroll
-            for (int c = 0; c < 2; c++)
-#pragma unroll
-              for (int t = 0; t < 4; t++) rt[(i0 + 8 * c) * PI + 4 * jg + t] = (int16_t)RI.stage2(acc[t][c]);
-          }
-        }
-      }
-      __syncthreads();
-      const int ls = ilog2(size), lr = ilog2(rep);
-      for (int p = tid; p < (size * size) >> 2; p += NT) {
-        int y = p >> (ls - 2), x = (p & ((size >> 2) - 1)) << 2;
-        int pv[4], ov[4], v[4];
-        load_row4<S>(pred + y * q.pstride + x, pv);
-        load_row4<S>(orig + y * q.ostride + x, ov);
-        const int16_t *rr = rt + (y >> lr) * PI;
-#pragma unroll
-        for (int t = 0; t < 4; t++) {
-          v[t] = sat_px((int)rr[(x + t) >> lr] + pv[t], maxv);
-          int d = ov[t] - v[t];
-          ssd += (uint64_t)(uint32_t)(d * d);
-        }
-        if (rec) store_row4<S>(rec + y * q.rstride + x, v);
-      }
-    } else {
-      for (int p = tid; p < core * core; p += NT) {
-        int i = p >> lc, j = p & (core - 1);
-        int sum = dot_s8_s16(Mt + j * mpc, tmp2 + i * PI, qsize);
-        int r = RI.stage2(sum);
-        for (int m = 0; m < rep; m++)
-          for (int nn = 0; nn < rep; nn++) {
-            int y = i * rep + m, x = j * rep + nn;
-            int v = sat_px(r + (int)(int16_t)pred[y * q.pstride + x], maxv);
-            if (rec) rec[y * q.rstride + x] = (S)v;
-            int d = (int)orig[y * q.ostride + x] - v;
-            ssd += (uint64_t)(uint32_t)(d * d);
-          }
-      }
-    }
-  } else {
-    // cbp == 0: the reference copies the prediction (enc/encode_block.c:1145-1166 "memcpy pred -> rec")
-    const int ls = ilog2(size);
-    for (int p = tid; p < (size * size) >> 2; p += NT) {
-      int y = p >> (ls - 2), x = (p & ((size >> 2) - 1)) << 2;
-      int pv[4], ov[4];
-      load_row4<S>(pred + y * q.pstride + x, pv);
-      load_row4<S>(orig + y * q.ostride + x, ov);
-      if (rec) store_row4<S>(rec + y * q.rstride + x, pv);
-#pragma unroll
-      for (int t = 0; t < 4; t++) { int d = ov[t] - pv[t]; ssd += (uint64_t)(uint32_t)(d * d); }
-    }
-  }
-  ssd = warp_sum64(ssd);
-  if (TW > 1) {
-    if (lane == 0) red[threadIdx.x >> 5] = ssd;
-    __syncthreads();
-    ssd = 0;
-#pragma unroll
-    for (int k = 0; k < TW; k++) ssd += red[k];
-  }
-  if (tid == 0) { res->ssd = ssd; res->cbp = cbp; res->bits = bits; }
-  sync();
-}
-
-// Scheduling as for the motion search (me_batch_kernel): blocks > 8x8 are listed largest first by the counting sort; the
-// persistent kernel (1) works through the 64x64 / 128x128 blocks as a CTA team, (2) gives the 16x16 / 32x32 blocks one warp
-// each, (3) draws groups of 32 consecutive items from the caller's array and runs their 4x4 and 8x8 blocks one per LANE
-// (thread_txfm4 in registers, thread_txfm8 in per-thread local arrays; consecutive items are spatial neighbours, so the
-// lanes' loads and stores coalesce).
+constexpr size_t TX_SMEM = TX_TABLE_BYTES + DCT_TAB_SIZE * sizeof(int16_t) + sizeof(TxWarp) * WARPS_PER_CTA;
 template <class S>
-__global__ void __launch_bounds__(CTA_THREADS, TX_MINBLOCKS) txfm_chain_kernel(const tb_txfm_item_t *items, int n, const int *idx, int *meta, int bitdepth, tb_txfm_result_t *out) {
+__global__ void __launch_bounds__(CTA_THREADS, TX_MINBLOCKS) txfm_chain_kernel(const tb_txfm_item_t *items, int n, int bitdepth, tb_txfm_result_t *out) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  __shared__ unsigned long long red[WARPS_PER_CTA];
-  __shared__ int bc, s_next;
-  int8_t *tab8 = (int8_t *)smem_raw, *tab8t = tab8 + DCT_TAB8_SIZE;
-  TxScratch *scs = (TxScratch *)(smem_raw + TX_TABLE_BYTES);
-  dct_tab8_fill(tab8, tab8t);
+  int8_t *tab8 = (int8_t *)smem_raw;
+  int16_t *tab16 = (int16_t *)(smem_raw + TX_TABLE_BYTES);
+  TxWarp &tw = ((TxWarp *)(smem_raw + TX_TABLE_BYTES + DCT_TAB_SIZE * sizeof(int16_t)))[threadIdx.x >> 5];
+  dct_tab8_fill(tab8, tab8 + DCT_TAB8_SIZE);
+  dct_tab_fill(tab16);
   for (int t = threadIdx.x; t < 256; t += blockDim.x) ((uint8_t *)(tab8 + 2 * DCT_TAB8_SIZE))[t] = (uint8_t)zigzag_index(t >> 4, t & 15, 16);
   __syncthreads();
-  const int lane = lane_id();
-  const int nteam = meta[96], nlisted = meta[99];
-  for (;;) {  // (1)
-    if (threadIdx.x == 0) s_next = atomicAdd(&meta[97], 1);
-    __syncthreads();
-    const int k = s_next;
-    __syncthreads();
-    if (k >= nteam) break;
-    const int it = idx[k];
-    tx_big_chain<S, WARPS_PER_CTA>(items[it], bitdepth, scs[0], scs[1].in, tab8, tab8t, red, &bc, out + it);
-  }
-  TxScratch &sc = scs[threadIdx.x >> 5];
-  for (;;) {  // (2)
-    int k = 0;
-    if (lane == 0) k = atomicAdd(&meta[98], 1);
-    k = nteam + __shfl_sync(FULL, k, 0);
-    if (k >= nlisted) break;
-    const int it = idx[k];
-    tx_big_chain<S, 1>(items[it], bitdepth, sc, nullptr, tab8, tab8t, nullptr, nullptr, out + it);
-  }
-  const int ngroups = (n + 31) >> 5;
-  for (;;) {  // (3)
-    int gidx = 0;
-    if (lane == 0) gidx = atomicAdd(&meta[100], 1);
-    gidx = __shfl_sync(FULL, gidx, 0);
-    if (gidx >= ngroups) break;
-    const int mine = gidx * 32 + lane;
-    int my_size = 0;
-    if (mine < n) my_size = items[mine].size;
-    if (my_size == 4) {
-      tb_txfm_item_t q = items[mine];
-      uint64_t ssd;
-      int bits;
-      int cbp = thread_txfm4<S>((const S *)q.orig, q.ostride, (const S *)q.pred, q.pstride, (S *)q.rec, q.rstride, q.coeffq, q.qp, q.coeff_type, bitdepth, ssd, q.fast & 2, bits);
-      out[mine].ssd = ssd; out[mine].cbp = cbp; out[mine].bits = bits;
-    } else if (my_size == 8) {
-      tb_txfm_item_t q = items[mine];
-      uint64_t ssd;
-      int bits;
-      int cbp = thread_txfm8<S>((const S *)q.orig, q.ostride, (const S *)q.pred, q.pstride, (S *)q.rec, q.rstride, q.coeffq, q.qp, q.coeff_type, bitdepth, tab8, tab8t, ssd,
-                                q.fast & 2, bits);
-      out[mine].ssd = ssd; out[mine].cbp = cbp; out[mine].bits = bits;
+  const int l = lane_id();
+  for (int b = global_warp() * TX_CHUNK; b < n; b += total_warps() * TX_CHUNK) {
+    const int nc = min(TX_CHUNK, n - b);
+    int key = -1;  // which call takes item b + l: 0 = tx_small, else tx_mid of this size and `fast` flag
+    if (l < nc) { const tb_txfm_item_t &q = items[b + l]; key = q.size <= 8 ? 0 : 2 * q.size + (q.fast & TB_TXFM_FAST); }
+    for (int k = 0, m; k < nc; k += m) {
+      const int kk = __shfl_sync(FULL, key, k);
+      m = min(__ffs(~(__ballot_sync(FULL, key == kk) >> k)) - 1, kk ? 4 : TX_CHUNK);  // the run of items k.. with this key
+      if (l < m) {
+        tb_txfm_item_t q = items[b + k + l];
+        if (!q.coeffq) q.coeffq = tw.lev + (l << (kk ? 8 : 6));
+        tw.jobs[l] = q;
+      }
+      __syncwarp();
+      int bit[TX_CHUNK];
+      if (kk) tx_mid<S>(tw.jobs, m, bit, tab8, tw.tiles, tw.jobs, bitdepth);
+      else tx_small<S>(tw.jobs, m, bit, tab16, tw.tiles, tw.jobs, bitdepth);
+      for (int t = 0; t < m; t++) {
+        const tb_txfm_item_t &q = tw.jobs[t];
+        const int size = q.size, qs = min(size, 16), lq = ilog2(qs);
+        const uint64_t ssd = warp_ssd<S>((const S *)q.orig, q.ostride, (const S *)q.rec, q.rstride, size, size);
+        int bits = 0;
+        if ((q.fast & TB_TXFM_BITS) && bit[t]) {  // the levels in scan order (the tiles are free after the chain)
+          for (int p = l; p < qs * qs; p += 32) tw.tiles[zigzag_index(p >> lq, p & (qs - 1), qs)] = q.coeffq[p];
+          __syncwarp();
+          bits = warp_coeff_bits(tw.tiles, qs * qs, size, q.coeff_type);
+          __syncwarp();
+        }
+        if (l == 0) out[b + k + t] = {ssd, bit[t], bits};
+      }
+      __syncwarp();
     }
-    __syncwarp();
   }
 }
 
 // drop-in single-shot kernels (one warp)
 __global__ void fwd_transform_kernel(const int16_t *block, int16_t *coeff, int size, int fast, int bitdepth) {
-  __shared__ TxShared sh;
+  __shared__ TxScratch sc;
   __shared__ int16_t tab[DCT_TAB_SIZE];
   dct_tab_fill(tab);
   __syncthreads();
   const int qsize = min(size, 16);
-  warp_fwd_transform(block, size, size, fast, bitdepth, sh.sc, sh.sc.rc, tab);
-  for (int p = lane_id(); p < qsize * qsize; p += 32) coeff[(p / qsize) * size + (p % qsize)] = sh.sc.rc[p];
+  warp_fwd_transform(block, size, size, fast, bitdepth, sc, sc.rc, tab);
+  for (int p = lane_id(); p < qsize * qsize; p += 32) coeff[(p / qsize) * size + (p % qsize)] = sc.rc[p];
 }
 __global__ void inv_transform_kernel(const int16_t *coeff, int16_t *block, int size, int bitdepth) {
-  __shared__ TxShared sh;
+  __shared__ TxScratch sc;
   __shared__ int16_t tab[DCT_TAB_SIZE];
   dct_tab_fill(tab);
   __syncthreads();
   const int qsize = min(size, 16);
-  for (int p = lane_id(); p < qsize * qsize; p += 32) sh.sc.rc[p] = coeff[(p / qsize) * size + (p % qsize)];
+  for (int p = lane_id(); p < qsize * qsize; p += 32) sc.rc[p] = coeff[(p / qsize) * size + (p % qsize)];
   __syncwarp();
-  warp_inv_transform(sh.sc.rc, qsize, size, bitdepth, sh.sc, block, size, tab);
+  warp_inv_transform(sc.rc, qsize, size, bitdepth, sc, block, size, tab);
 }
 __global__ void quant_kernel(const int16_t *coeff, int16_t *coeffq, int qp, int size, int type, int32_t *cbp) {
-  __shared__ TxShared sh;
+  __shared__ TxScratch sc;
   const int qsize = min(size, 16);
-  for (int p = lane_id(); p < qsize * qsize; p += 32) sh.sc.rc[p] = coeff[(p / qsize) * size + (p % qsize)];
+  for (int p = lane_id(); p < qsize * qsize; p += 32) sc.rc[p] = coeff[(p / qsize) * size + (p % qsize)];
   __syncwarp();
-  int c = warp_quantize(sh.sc.rc, sh.sc.cq, qp, size, type, sh.sc);
-  for (int p = lane_id(); p < qsize * qsize; p += 32) coeffq[p] = sh.sc.cq[p];
+  int c = warp_quantize(sc.rc, sc.cq, qp, size, type, sc);
+  for (int p = lane_id(); p < qsize * qsize; p += 32) coeffq[p] = sc.cq[p];
   if (lane_id() == 0) *cbp = c;
 }
 __global__ void dequant_kernel(const int16_t *coeffq, int16_t *rcoeff, int qp, int size) {
-  __shared__ TxShared sh;
+  __shared__ TxScratch sc;
   const int qsize = min(size, 16);
-  warp_dequantize(coeffq, sh.sc.rc, qp, size);
-  for (int p = lane_id(); p < qsize * qsize; p += 32) rcoeff[(p / qsize) * size + (p % qsize)] = sh.sc.rc[p];
+  warp_dequantize(coeffq, sc.rc, qp, size);
+  for (int p = lane_id(); p < qsize * qsize; p += 32) rcoeff[(p / qsize) * size + (p % qsize)] = sc.rc[p];
 }
 __global__ void calc_cbp_kernel(const int16_t *block, int size, int thr, int32_t *res) {
   int r = warp_calc_cbp(block, size, thr);

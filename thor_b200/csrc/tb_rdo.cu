@@ -6,8 +6,8 @@
 // (reconstruction, per-4x4 block state, the leaf list of every super block with its coefficients).
 // The control flow is tb_rdo.h (shared with the CPU host check that pins it against the reference); this file supplies its backend:
 // the warp-cooperative primitives of tb_device.cuh, the same device routines the batched tb_* entry points and the drop-in symbols
-// use (parity-tested against the oracle one by one in tests/test_gpu_parity.py), and the RD loop's own loop forms of the transform
-// chain (tx_small, tx_mid), which take their arithmetic from the same a10-a13 rules.
+// use (parity-tested against the oracle one by one in tests/test_gpu_parity.py); its transform chains are tx_small and tx_mid,
+// which tb_txfm_chain_batch runs too.
 //
 // This is a separate translation unit because two load policies differ from the batched kernels:
 //   TB_LDG -> plain load: the "original" of a search can be a scratch block this CTA wrote a moment ago (bipred target 2*org - pred),
@@ -74,11 +74,10 @@ struct RdoCta {
   unsigned long long t_sb;  // %globaltimer when the current super block started
 };
 // per-warp scratch
-constexpr int TX_TILES = 3584;  // int16 tiles of the 16x16 to 128x128 chains (tx_mid), in the space of the other transform forms' scratch
 template <class S> struct RdoShared {
   long long prof[ST_END];
   long long t_mark, t_mark2;
-  alignas(16) unsigned char jobs[12 * 64];  // tx_multi: the chains' parameters
+  alignas(16) unsigned char jobs[12 * 64];  // tx_multi: the job area of tx_small / tx_mid (12 tb_txfm_item_t)
   union {
     struct {
       TxScratch sc;
@@ -88,6 +87,7 @@ template <class S> struct RdoShared {
     alignas(16) int16_t tiles[TX_TILES];
   };
   static_assert(TX_TILES * sizeof(int16_t) <= sizeof(TxScratch) + 2 * 256 * sizeof(int16_t), "the tiles take no shared memory of their own");
+  static_assert(12 * sizeof(tb_txfm_item_t) <= sizeof(jobs), "job area");
   alignas(16) S left[256], top[256], filt[4 * 128 + 4];
 };
 
@@ -282,256 +282,22 @@ template <class S> struct DevBackend {
     sync();
   }
   __device__ __noinline__ int tx_chain(const S *orig, int os, const S *pred, int ps, S *rec, int rs, int16_t *cq, int size, int qp, int coeff_type, int fast) const {
-    tbr::TxJob<S> j;
-    j.orig = orig; j.pred = pred; j.rec = rec; j.cq = cq; j.os = os; j.ps = ps; j.rs = rs; j.size = size; j.qp = qp; j.coeff_type = coeff_type; j.fast = fast;
+    tb_txfm_item_t j;
+    j.orig = orig; j.pred = pred; j.rec = rec; j.coeffq = cq; j.ostride = os; j.pstride = ps; j.rstride = rs;
+    j.size = (uint8_t)size; j.qp = (uint8_t)qp; j.coeff_type = (uint8_t)coeff_type; j.fast = (uint8_t)fast;
     int cbp;
     tx_multi(&j, 1, &cbp);
     return cbp;
   }
   // chains of one transform size (4x4 and 8x8 may mix), in the order of the list; bit[k] = cbp of chain k
-  __device__ __noinline__ void tx_multi(const tbr::TxJob<S> *jobs, int n, int *bit) const {
-    if (jobs[0].size <= 8) tx_small(jobs, n, bit);
-    else tx_mid(jobs, n, bit);
-  }
-  // m . v over 16 * nc terms (int8 matrix row, int16 vector; both 16-byte aligned)
-  __device__ __forceinline__ static int dot_rows(const int8_t *m, const int16_t *v, int nc) {
-    int acc[1][1] = {{0}};
-    TB_ROLL
-    for (int c = 0; c < nc; c++) dot16_block<1, 1>(m + 16 * c, 0, v + 16 * c, 0, acc);
-    return acc[0][0];
-  }
-  // <= 12 chains of 16x16 to 128x128 transform blocks, all of the same size and `fast` flag: the 16- or 32-point forward transform of the s1 x s1
-  // box sums of the residual (BoxSum), 16x16 coefficients, and the inverse on a core of min(N, 32) points whose every output a block larger than
-  // 32x32 replicates rep x rep (common/transform.c:481-492).  Written, like tx_small, as LOOPS over (chain, element) work items dealt to the lanes,
-  // one output per item with the 16-term DP2A dot product of dot16_block, so that the code stays a few KB.  The chains of a group share every
-  // stage: four with s1 = 16 (16x16, and every size with `fast`), one with s1 = 32, in the TX_TILES int16 of the warp's scratch.  Per chain two tiles:
-  //   X: box sums (s1 x s1, pitch p1) -> coefficients in scan order, quantised in place (256) -> inverse first stage, transposed (core x 16)
-  //   Y: forward first stage (16 x s1, pitch p1) -> dequantised coefficients, transposed (16 x 16, pitch 24)
-  // Pitches of tiles whose rows the lanes of a quarter-warp read side by side are 48 or 80 bytes: conflict-free 128-bit loads.  The quantiser's
-  // level-mode walk stays warp-parallel (warp_quantize_scan), one chain after the other.
-  __device__ __noinline__ void tx_mid(const tbr::TxJob<S> *jobs, int n, int *bit) const {
-    const int N = jobs[0].size, ln = ilog2(N);
-    const BoxSum B(N, jobs[0].fast);
-    const int s1 = B.size1, l1 = ilog2(s1), p1 = s1 + 8, core = min(N, 32), lc = ilog2(core), lr = ln - lc;
-    PROF2(PF_TX, ST_TX_SZ + ln - 2);
-    const int l = lane();
-    if (l == 0) { sh->prof[ST_TX] += n; sh->prof[ST_TX_SAMPLES] += 3 * n * N * N; }
-    tbr::TxJob<S> *J = (tbr::TxJob<S> *)sh->jobs;
-    sync();
-    if (l < n) J[l] = jobs[l];
-    sync();
-    const int xs = max(s1 * p1, core * 16), cs = xs + 16 * p1, g = TX_TILES / cs;
-    const int bd = F->bitdepth, maxv = (1 << bd) - 1;
-    const int8_t *M1 = cta->tab8 + dct_tab8_ofs(l1), *Mt = cta->tab8 + DCT_TAB8_SIZE + dct_tab8_ofs(lc);
-    const uint8_t *zz16 = (const uint8_t *)(cta->tab8 + 2 * DCT_TAB8_SIZE);
-    const FwdRound R(ln, B.log2scale, bd);
-    const InvRound RI(bd);
-    int16_t *T = sh->tiles;
-    TB_ROLL
-    for (int k0 = 0; k0 < n; k0 += g) {
-      const int m = min(g, n - k0);
-      const tbr::TxJob<S> *G = J + k0;
-      // (1) residual -> X[k][i][j], the box sums
-      TB_ROLL
-      for (int w = l; w < (m << (2 * l1)); w += 32) {
-        const int k = w >> (2 * l1), e = w & ((1 << (2 * l1)) - 1), i = e >> l1, j = e & (s1 - 1);
-        const tbr::TxJob<S> &q = G[k];
-        T[k * cs + i * p1 + j] = B(i, j, [&](int y, int x) { return (int)q.orig[y * q.os + x] - (int)q.pred[y * q.ps + x]; });
-      }
-      sync();
-      // (2) forward, first dimension: Y[k][i][j] = stage1(M[i][.] . X[k][j][.])   (i < 16, j < s1)
-      TB_ROLL
-      for (int w = l; w < (m << (4 + l1)); w += 32) {
-        const int k = w >> (4 + l1), e = w & ((16 << l1) - 1), i = e >> l1, j = e & (s1 - 1);
-        T[k * cs + xs + i * p1 + j] = (int16_t)R.stage1(dot_rows(M1 + (i << l1), T + k * cs + j * p1, s1 >> 4));
-      }
-      sync();
-      // (3) forward, second dimension, to X[k] in scan order: X[k][zz(i, j)] = stage2(M[i][.] . Y[k][j][.])   (i, j < 16)
-      TB_ROLL
-      for (int w = l; w < (m << 8); w += 32) {
-        const int k = w >> 8, e = w & 255, i = e >> 4, j = e & 15;
-        T[k * cs + zz16[e]] = (int16_t)R.stage2(dot_rows(M1 + (i << l1), T + k * cs + xs + j * p1, s1 >> 4));
-      }
-      sync();
-      // (4) quantiser, in place, one chain after the other
-      unsigned nz = 0;
-      TB_ROLL
-      for (int k = 0; k < m; k++) {
-        const tbr::TxJob<S> &q = G[k];
-        nz |= (unsigned)warp_quantize_scan(T + k * cs, T + k * cs, 256, Quantizer(q.qp, ln, q.coeff_type)) << k;
-      }
-      // (5) levels, raster, to the caller's buffer (reference layout) and, dequantised, transposed to Y[k][j][i] = rcoeff[i][j] (pitch 24)
-      TB_ROLL
-      for (int w = l; w < (m << 8); w += 32) {
-        const int k = w >> 8, e = w & 255;
-        const tbr::TxJob<S> &q = G[k];
-        const int c = T[k * cs + zz16[e]];
-        q.cq[e] = (int16_t)c;
-        T[k * cs + xs + (e & 15) * 24 + (e >> 4)] = (int16_t)Dequantizer(q.qp, ln)(c);
-      }
-      sync();
-      // (6) inverse, first dimension: X[k][j][i] = stage1(sum_t M[t][j] * rcoeff[t][i])   (j < core, i < 16; pitch 16)
-      TB_ROLL
-      for (int w = l; w < (m << (lc + 4)); w += 32) {
-        const int k = w >> (lc + 4), e = w & ((16 << lc) - 1), j = e >> 4, i = e & 15;
-        if ((nz >> k) & 1) T[k * cs + e] = (int16_t)InvRound::stage1(dot_rows(Mt + (j << lc), T + k * cs + xs + i * 24, 1));
-      }
-      sync();
-      // (7) inverse, second dimension + reconstruction of the rep x rep samples of core output (i, j) (i, j < core):
-      // rec = clip(pred + stage2(sum_t M[t][j] * X[k][i][t])); no coefficient: rec = pred
-      TB_ROLL
-      for (int w = l; w < (m << (2 * lc)); w += 32) {
-        const int k = w >> (2 * lc), e = w & ((1 << (2 * lc)) - 1), i = e >> lc, j = e & (core - 1);
-        const tbr::TxJob<S> &q = G[k];
-        const bool c = (nz >> k) & 1;
-        const int r = c ? RI.stage2(dot_rows(Mt + (j << lc), T + k * cs + i * 16, 1)) : 0;
-        TB_ROLL
-        for (int t = 0; t < (1 << (2 * lr)); t++) {
-          const int y = (i << lr) + (t >> lr), x = (j << lr) + (t & ((1 << lr) - 1));
-          const int v = (int)q.pred[y * q.ps + x];
-          q.rec[y * q.rs + x] = (S)(c ? sat_px(v + r, maxv) : v);
-        }
-      }
-      sync();
-      TB_ROLL
-      for (int k = 0; k < m; k++) bit[k0 + k] = (nz >> k) & 1;
-    }
-  }
-  // <= 12 chains of 4x4 / 8x8 transform blocks (residual -> DCT -> quantiser -> dequantiser -> inverse DCT -> reconstruction, the arithmetic of
-  // common/transform.c:245-308, 411-494, enc/encode_block.c:84-171, common/common_block.c:45-83), all of them together on the warp.  Written as LOOPS over
-  // (chain, element) work items dealt to the lanes: the RD loop is bound by instruction fetch, so a few hundred instructions that stay in the instruction cache beat the unrolled one-thread-per-chain forms (5.6 k instructions
-  // streamed from L2 per call).  Tiles of 64 int16 per chain in the warp's scratch; the quantiser's level-mode walk is sequential: one lane per chain.
-  __device__ __noinline__ void tx_small(const tbr::TxJob<S> *jobs, int n, int *bit) const {
+  __device__ __noinline__ void tx_multi(const tb_txfm_item_t *jobs, int n, int *bit) const {
     PROF2(PF_TX, ST_TX_SZ + ilog2(jobs[0].size) - 2);
-    const int l = lane();
-    if (l == 0)
+    if (lane() == 0)
       TB_ROLL
       for (int k = 0; k < n; k++) { sh->prof[ST_TX] += 1; sh->prof[ST_TX_SAMPLES] += 3 * jobs[k].size * jobs[k].size; }
-    int16_t *A = sh->sc.in, *B = sh->sc.in + 768;  // 12 tiles of 64 each
-    // chain parameters in shared memory (per warp): the loops index them by chain
-    tbr::TxJob<S> *J = (tbr::TxJob<S> *)sh->jobs;
-    sync();
-    if (l < n) J[l] = jobs[l];
-    sync();
-    const int bd = F->bitdepth, maxv = (1 << bd) - 1;
-    // (1) residual -> A[k][i * N + j]
-    TB_ROLL
-    for (int w = l; w < n * 64; w += 32) {
-      const int k = w >> 6, e = w & 63;
-      const tbr::TxJob<S> &q = J[k];
-      const int N = q.size, ln = N == 8 ? 3 : 2;
-      if (e < N * N) { const int i = e >> ln, j = e & (N - 1); A[w] = (int16_t)((int)q.orig[i * q.os + j] - (int)q.pred[i * q.ps + j]); }
-    }
-    sync();
-    // (2) forward, first dimension: B[k][i][j] = stage1(sum_t M[i][t] * A[k][j][t])
-    TB_ROLL
-    for (int w = l; w < n * 64; w += 32) {
-      const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
-      if (e < N * N) {
-        const int i = e >> ln, j = e & (N - 1);
-        const int16_t *M = cta->tab16 + (N == 8 ? 16 : 0) + (i << ln), *a = A + (k << 6) + (j << ln);
-        int sum = 0;
-        TB_ROLL
-        for (int t = 0; t < N; t++) sum += (int)M[t] * (int)a[t];
-        B[w] = (int16_t)FwdRound(ln, 0, bd).stage1(sum);
-      }
-    }
-    sync();
-    // (3) forward, second dimension: A[k][i][j] = stage2(sum_t M[i][t] * B[k][j][t])   (coefficients, raster)
-    TB_ROLL
-    for (int w = l; w < n * 64; w += 32) {
-      const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
-      int v = 0;
-      if (e < N * N) {
-        const int i = e >> ln, j = e & (N - 1);
-        const int16_t *M = cta->tab16 + (N == 8 ? 16 : 0) + (i << ln), *b = B + (k << 6) + (j << ln);
-        int sum = 0;
-        TB_ROLL
-        for (int t = 0; t < N; t++) sum += (int)M[t] * (int)b[t];
-        v = FwdRound(ln, 0, bd).stage2(sum);
-      }
-      if (e < N * N) A[w] = (int16_t)v;  // A was consumed by (2)
-    }
-    sync();
-    // (4) zig-zag scan order -> B[k][pos]
-    TB_ROLL
-    for (int w = l; w < n * 64; w += 32) {
-      const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
-      if (e < N * N) B[(k << 6) + zigzag_index(e >> ln, e & (N - 1), N)] = A[w];
-    }
-    sync();
-    // (5) quantiser (sequential level-mode walk), lane k on chain k: levels in scan order -> B[k][pos] in place; cbp
-    int cbp = 0;
-    if (l < n) {
-      const tbr::TxJob<S> &q = J[l];
-      const int N = q.size, nq = N * N;
-      const Quantizer Q(q.qp, N == 8 ? 3 : 2, q.coeff_type);
-      int16_t *sc_ = B + (l << 6);
-      bool nz = false;
-      int pos = nq - 1;
-      while (!nz && pos >= 0) nz = Q.last_nz(sc_[pos--]);
-      const int last_pos = nz ? pos + 1 : pos;
-      int level_mode = 1;
-      TB_ROLL
-      for (pos = 0; pos <= last_pos; pos++) {
-        const int c = sc_[pos], lev = Q.level(c, level_mode);
-        sc_[pos] = (int16_t)(c < 0 ? -lev : lev);
-        cbp |= lev != 0;
-        level_mode = Quantizer::next_mode(level_mode, lev);
-      }
-      TB_ROLL
-      for (pos = last_pos + 1; pos < nq; pos++) sc_[pos] = 0;
-    }
-    sync();
-    const unsigned nzmask = __ballot_sync(FULL, cbp != 0);
-    // (6) quantised coefficients, raster: to the caller's buffer (reference layout) and, dequantised, to A[k] (dequantize(), common/common_block.c:45)
-    TB_ROLL
-    for (int w = l; w < n * 64; w += 32) {
-      const int k = w >> 6, e = w & 63;
-      const tbr::TxJob<S> &q = J[k];
-      const int N = q.size, ln = N == 8 ? 3 : 2;
-      if (e < N * N) {
-        const int c = B[(k << 6) + zigzag_index(e >> ln, e & (N - 1), N)];
-        q.cq[e] = (int16_t)c;
-        A[w] = (int16_t)Dequantizer(q.qp, ln)(c);
-      }
-    }
-    sync();
-    // (7) inverse, first dimension: B[k][i][j] = stage1(sum_t M[t][j] * A[k][t][i])
-    TB_ROLL
-    for (int w = l; w < n * 64; w += 32) {
-      const int k = w >> 6, e = w & 63, N = J[k].size, ln = N == 8 ? 3 : 2;
-      if (e < N * N && ((nzmask >> k) & 1)) {
-        const int i = e >> ln, j = e & (N - 1);
-        const int16_t *M = cta->tab16 + (N == 8 ? 16 : 0), *a = A + (k << 6);
-        int o = 0;
-        TB_ROLL
-        for (int t = 0; t < N; t++) o += (int)M[(t << ln) + j] * (int)a[(t << ln) + i];
-        B[w] = (int16_t)InvRound::stage1(o);
-      }
-    }
-    sync();
-    // (8) inverse, second dimension + reconstruction: rec = clip(pred + stage2(sum_t M[t][j] * B[k][t][i])); no coefficient: rec = pred
-    TB_ROLL
-    for (int w = l; w < n * 64; w += 32) {
-      const int k = w >> 6, e = w & 63;
-      const tbr::TxJob<S> &q = J[k];
-      const int N = q.size, ln = N == 8 ? 3 : 2;
-      if (e < N * N) {
-        const int i = e >> ln, j = e & (N - 1);
-        int v = (int)q.pred[i * q.ps + j];
-        if ((nzmask >> k) & 1) {
-          const int16_t *M = cta->tab16 + (N == 8 ? 16 : 0), *b = B + (k << 6);
-          int o = 0;
-          TB_ROLL
-          for (int t = 0; t < N; t++) o += (int)M[(t << ln) + j] * (int)b[(t << ln) + i];
-          v = sat_px(v + InvRound(bd).stage2(o), maxv);
-        }
-        q.rec[i * q.rs + j] = (S)v;
-      }
-    }
-    sync();
-    for (int k = 0; k < n; k++) bit[k] = (nzmask >> k) & 1;
+    tb_txfm_item_t *J = (tb_txfm_item_t *)sh->jobs;
+    if (jobs[0].size <= 8) tx_small<S>(jobs, n, bit, cta->tab16, sh->tiles, J, F->bitdepth);
+    else tx_mid<S>(jobs, n, bit, cta->tab8, sh->tiles, J, F->bitdepth);
   }
   __device__ __noinline__ int coeff_bits(const int16_t *cq, int size, int type) const {
     PROF(PF_BITS);

@@ -153,12 +153,6 @@ struct Cand {
   int cbp_y, cbp_u, cbp_v;
   int tb_param, tb_split;
 };
-// one transform chain of a candidate (residual -> DCT -> quant -> dequant -> inverse DCT -> reconstruction): the chains of a candidate's planes and
-// transform blocks are independent of each other when the predictions are complete, so the backend may run them side by side (tx_multi)
-template <class S> struct TxJob {
-  const S *orig; const S *pred; S *rec; int16_t *cq;
-  int os, ps, rs, size, qp, coeff_type, fast;
-};
 // block_info_t
 struct BlockInfo {
   int size, ypos, xpos, bwidth, bheight;
@@ -441,23 +435,24 @@ template <class S, class B> struct Rdo {
   // the fast flag of the inter transform chains of a size x size block (encode_and_reconstruct_block_inter :1275-1338)
   TBR_HD int inter_fast(int size, int tb_split) const { return tb_split ? size == 64 || F.speed > 1 : (size == 64 && F.speed > 0) || F.speed > 1; }
   // the transform chains of encode_and_reconstruct_block_inter :1275-1338 for one plane (orig/pred/rec compact or strided; coefficients in the
-  // reference layout), appended to a job list in the reference's order; returns the number of chains
-  TBR_HD int inter_jobs(TxJob<S> *jobs, const S *orig, int os, int size, int qp, const S *pred, int16_t *cq, S *rec, int coeff_type, int tb_split) const {
+  // reference layout), appended to a job list in the reference's order; returns the number of chains.  The chains of a candidate's planes and
+  // transform blocks are independent of each other when the predictions are complete, so the backend may run them side by side (tx_multi).
+  TBR_HD int inter_jobs(tb_txfm_item_t *jobs, const S *orig, int os, int size, int qp, const S *pred, int16_t *cq, S *rec, int coeff_type, int tb_split) const {
     if (tb_split) {
       const int s2 = size / 2;
       int n = 0;
       for (int i = 0; i < size; i += s2)
         for (int j = 0; j < size; j += s2) {
-          TxJob<S> &q = jobs[n];
-          q.orig = orig + i * os + j; q.os = os; q.pred = pred + i * size + j; q.ps = size; q.rec = rec + i * size + j; q.rs = size; q.cq = cq + 256 * n; q.size = s2; q.qp = qp;
-          q.coeff_type = coeff_type; q.fast = inter_fast(size, 1);
+          tb_txfm_item_t &q = jobs[n];
+          q.orig = orig + i * os + j; q.ostride = os; q.pred = pred + i * size + j; q.pstride = size; q.rec = rec + i * size + j; q.rstride = size;
+          q.coeffq = cq + 256 * n; q.size = (uint8_t)s2; q.qp = (uint8_t)qp; q.coeff_type = (uint8_t)coeff_type; q.fast = (uint8_t)inter_fast(size, 1);
           n++;
         }
       return 4;
     }
-    TxJob<S> &q = jobs[0];
-    q.orig = orig; q.os = os; q.pred = pred; q.ps = size; q.rec = rec; q.rs = size; q.cq = cq; q.size = size; q.qp = qp; q.coeff_type = coeff_type;
-    q.fast = inter_fast(size, 0);
+    tb_txfm_item_t &q = jobs[0];
+    q.orig = orig; q.ostride = os; q.pred = pred; q.pstride = size; q.rec = rec; q.rstride = size; q.coeffq = cq; q.size = (uint8_t)size; q.qp = (uint8_t)qp;
+    q.coeff_type = (uint8_t)coeff_type; q.fast = (uint8_t)inter_fast(size, 0);
     return 1;
   }
   TBR_HD static int join_cbp(const int *bit, int n) {
@@ -488,10 +483,13 @@ template <class S, class B> struct Rdo {
   TBR_HD TBR_NI void uv_chains(const S *ou, const S *ov, int os, const S *pu, const S *pv, int ps, S *ru, S *rv, int rs, int16_t *cqu, int16_t *cqv, int size, int qp, int coeff_type,
                         int fast, int *bu, int *bv) {
     if (size <= 16) {
-      TxJob<S> jobs[2];
+      tb_txfm_item_t jobs[2];
       int bit[2];
-      jobs[0].orig = ou; jobs[0].pred = pu; jobs[0].rec = ru; jobs[0].cq = cqu; jobs[1].orig = ov; jobs[1].pred = pv; jobs[1].rec = rv; jobs[1].cq = cqv;
-      for (int k = 0; k < 2; k++) { jobs[k].os = os; jobs[k].ps = ps; jobs[k].rs = rs; jobs[k].size = size; jobs[k].qp = qp; jobs[k].coeff_type = coeff_type; jobs[k].fast = fast; }
+      jobs[0].orig = ou; jobs[0].pred = pu; jobs[0].rec = ru; jobs[0].coeffq = cqu; jobs[1].orig = ov; jobs[1].pred = pv; jobs[1].rec = rv; jobs[1].coeffq = cqv;
+      for (int k = 0; k < 2; k++) {
+        jobs[k].ostride = os; jobs[k].pstride = ps; jobs[k].rstride = rs;
+        jobs[k].size = (uint8_t)size; jobs[k].qp = (uint8_t)qp; jobs[k].coeff_type = (uint8_t)coeff_type; jobs[k].fast = (uint8_t)fast;
+      }
       be.tx_multi(jobs, 2, bit);
       *bu = bit[0]; *bv = bit[1];
     } else {
@@ -554,10 +552,10 @@ template <class S, class B> struct Rdo {
         be.copy(W.rec_v, sizeC, W.p_v, sizeC, sizeC, sizeC);
         c.cbp_y = c.cbp_u = c.cbp_v = 0;
       } else {
-        TxJob<S> jobs[12];
+        tb_txfm_item_t jobs[12];
         int bit[12];
         if (!F.cfl_inter && sizeC <= 8) {
-          // small blocks: the chains of the three planes (<= 12 of 4x4 / 8x8, one thread each on the device) side by side; a 16x16 luma block goes first, alone
+          // small blocks: the chains of the three planes (<= 12 of 4x4 / 8x8) side by side; a 16x16 luma block goes first, alone
           int n = 0, ny = 0;
           const int tbc = tb_split && sizeC > 4;
           if (size == 16 && !tb_split) c.cbp_y = be.tx_chain(oy, F.org_stride[0], W.p_y, size, W.rec_y, size, W.cq_y, size, F.qp, itype | 0, inter_fast(size, 0));

@@ -183,7 +183,7 @@ def tu_list(cfg, blocks):
     return np.concatenate(rows).astype(np.int32)
 
 
-def build_txfm(cfg, R, tus, planes_cur, planes_ref, planes_rec, rng):
+def build_txfm(cfg, R, tus, planes_cur, planes_ref, rec_ptr, rng):
     n, ESZ = len(tus), cfg.ESZ
     size, x, y, chroma = tus[:, 0], tus[:, 1], tus[:, 2], tus[:, 3]
     items = np.zeros(n, R.TXFM_ITEM)
@@ -192,12 +192,11 @@ def build_txfm(cfg, R, tus, planes_cur, planes_ref, planes_rec, rng):
     dx = rng.integers(-3, 4, n); dy = rng.integers(-3, 4, n)  # prediction = displaced reference block
     items["orig"] = cp + (y.astype(np.uint64) * cs.astype(np.uint64) + x.astype(np.uint64)) * np.uint64(ESZ)
     items["pred"] = (rp.astype(np.int64) + ((y + dy).astype(np.int64) * rs + (x + dx)) * ESZ).astype(np.uint64)
-    if planes_rec is not None:
-        op = np.array([planes_rec[0][0], planes_rec[1][0]], np.uint64)[chroma]; os_ = np.array([planes_rec[0][1], planes_rec[1][1]])[chroma]
-        items["rec"] = op + (y.astype(np.uint64) * os_.astype(np.uint64) + x.astype(np.uint64)) * np.uint64(ESZ)
-        items["rstride"] = os_
-    # else rec = NULL: the reconstruction goes to a private scratch block (CPU arm: candidates of one block would otherwise race on the
-    # shared plane between threads and make the SSD read-back nondeterministic; the GPU kernel takes the SSD from registers)
+    if rec_ptr is not None:  # every candidate reconstructs into a block of its own: the kernel reads it back for the SSD
+        ofs = np.concatenate([[0], np.cumsum(size.astype(np.int64) ** 2)[:-1]]).astype(np.uint64)
+        items["rec"] = np.uint64(rec_ptr) + ofs * np.uint64(ESZ)
+        items["rstride"] = size
+    # else rec = NULL: the CPU replay reconstructs into a private scratch block per thread
     items["coeffq"] = 0
     items["ostride"] = cs; items["pstride"] = rs
     items["size"] = size; items["qp"] = np.where(chroma == 1, cfg.QPC, cfg.QP)
@@ -305,13 +304,13 @@ class Workload:
         _, self.ip_total, _ = interp_geometry(cfg, self.blocks)
         _, self.in_total = intra_geometry(cfg, self.blocks)
 
-    def bind(self, cur_planes, ref_planes, rec_plane0, cand_rec_planes, pred_ptr, intra_ptr):
-        """cur_planes: [(ptr, stride)] x 2 (Y, U); ref_planes: [[(ptr, stride)] x 3] x NREF; rec_plane0: (ptr, stride); cand_rec_planes:
-        [(ptr, stride)] x 2 or None"""
+    def bind(self, cur_planes, ref_planes, rec_plane0, cand_rec_ptr, pred_ptr, intra_ptr):
+        """cur_planes: [(ptr, stride)] x 2 (Y, U); ref_planes: [[(ptr, stride)] x 3] x NREF; rec_plane0: (ptr, stride); cand_rec_ptr:
+        tx_samples() samples for the candidates' reconstructions, or None"""
         cfg, R = self.cfg, self.R
         rng = np.random.default_rng([self.seed, 2])
         self.me, self.cands = build_me(cfg, R, self.blocks, cur_planes[0], [r[0] for r in ref_planes], rng)
-        self.tx = build_txfm(cfg, R, self.tus, cur_planes, [ref_planes[0][0], ref_planes[0][1]], cand_rec_planes, rng)
+        self.tx = build_txfm(cfg, R, self.tus, cur_planes, [ref_planes[0][0], ref_planes[0][1]], cand_rec_ptr, rng)
         self.ip = build_interp(cfg, R, self.blocks, ref_planes, pred_ptr, rng)
         self.intra = build_intra(cfg, R, self.blocks, rec_plane0, intra_ptr)
         self.bi = build_blkinfo(cfg, R, rng)
@@ -321,6 +320,9 @@ class Workload:
 
     def counts(self):
         return len(self.me), len(self.ip), len(self.tx), len(self.intra)
+
+    def tx_samples(self):
+        return int((self.tus[:, 0].astype(np.int64) ** 2).sum())
 
     def txfm_alg_bytes(self):
         """SURVEY.md §8d for the chain: orig + pred read, rec written (3 N^2 s) + the 48-byte item + the 16-byte result"""
@@ -431,12 +433,11 @@ def run_gpu(args, cfg):
         refs.append(r)
     pristine = tb.Frame(W, H, ESZ); pristine.upload(*fr[1])  # un-filtered reconstruction, restored device-side every step
     rec = tb.Frame(W, H, ESZ); rec.upload(*fr[1]); scratch = tb.Frame(W, H, ESZ); newref = tb.Frame(W, H, ESZ)
-    cand_rec = tb.Frame(W, H, ESZ)  # where RD candidates write their reconstructions
 
     wl = Workload(cfg, tb, seed)
     pred_buf = tb.DevBuf(wl.ip_total * ESZ + 64); intra_buf = tb.DevBuf(wl.in_total * ESZ + 64)
-    wl.bind([cur.plane(0), cur.plane(1)], [[r.plane(p) for p in range(3)] for r in refs], rec.plane(0), [cand_rec.plane(0), cand_rec.plane(1)],
-            pred_buf.ptr, intra_buf.ptr)
+    cand_rec = tb.DevBuf(wl.tx_samples() * ESZ)  # where RD candidates write their reconstructions
+    wl.bind([cur.plane(0), cur.plane(1)], [[r.plane(p) for p in range(3)] for r in refs], rec.plane(0), cand_rec.ptr, pred_buf.ptr, intra_buf.ptr)
     me_items, cands, tx_items, ip_items, in_items = wl.me, wl.cands, wl.tx, wl.ip, wl.intra
     nfb = ((W + 63) // 64) * ((H + 63) // 64)
 
