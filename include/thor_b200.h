@@ -296,15 +296,25 @@ int tb_rdo_encode_frame(const tb_rdo_frame_t *f);
  * have the same sample size; geometry and parameters may differ.  Same outputs per frame as tb_rdo_encode_frame(). */
 int tb_rdo_encode_frames(const tb_rdo_frame_t *f, int n);
 /* The same in steps, for callers that keep frames resident or overlap the copies: every call only ENQUEUES on the library's stream
- * (tb_stream()); host buffers must stay valid until tb_rdo_batch_sync() (pinned buffers make the copies truly asynchronous). */
+ * (tb_stream()); host buffers must stay valid until tb_rdo_batch_sync() (pinned buffers make the copies truly asynchronous).
+ * Any sequence of calls may be enqueued before one sync, e.g. upload A, run, download A, upload B into the same slots, run, download B, sync: each
+ * launch reads the uploads enqueued before it and each download returns the launch enqueued before it.  The host waits only where it must:
+ *   - an upload into a slot whose previous upload's copies have not started yet waits for them (the frame parameters are staged per slot);
+ *   - an upload that changes a slot's geometry (size, super-block size, sample size, reference padding or stride, or more than five references)
+ *     reallocates it and first waits for the stream to drain; so does a run that needs more rows, super blocks or CTAs than any launch before;
+ *   - a run with eight launches of the batch in flight waits for the oldest of them.
+ * A run over [0, n_active) leaves slots >= n_active untouched: their downloads return the decisions of the last launch that included them, until
+ * an upload changes their geometry. */
 typedef struct tb_rdo_batch tb_rdo_batch_t;
 tb_rdo_batch_t *tb_rdo_batch_create(int n_slots, int sample_bytes);                         /* NULL: tb_rdo_last_error() */
 int tb_rdo_batch_upload(tb_rdo_batch_t *b, int slot, const tb_rdo_frame_t *f);              /* parameters + source + references -> HBM */
 int tb_rdo_batch_run(tb_rdo_batch_t *b, int n_active);                                      /* one launch over slots [0, n_active) */
 int tb_rdo_batch_download(tb_rdo_batch_t *b, int slot, const tb_rdo_frame_t *f);            /* decisions of a slot -> f's output buffers (rec[] may be NULL) */
-int tb_rdo_batch_sync(tb_rdo_batch_t *b);                                                   /* waits; TB_ERR_CUDA if the launch did not finish every super block */
+int tb_rdo_batch_sync(tb_rdo_batch_t *b);                                                   /* waits; TB_ERR_CUDA if any launch since the previous sync did not
+                                                                                               finish every super block */
 int tb_rdo_batch_grid(const tb_rdo_batch_t *b);                                             /* CTAs of the last launch */
-/* counters of the last synchronised launch, summed over all warps: [0..10] SM cycles per primitive class (interp, search, bipred search, transform
+/* Stats and trace describe the last launch of the batch and are read after tb_rdo_batch_sync().
+ * counters of the last synchronised launch, summed over all warps: [0..10] SM cycles per primitive class (interp, search, bipred search, transform
  * chain, coefficient bits, SSD/SAD, intra, copies, early skip, idle, total); [11..22] work actually executed (the RD loop is data dependent):
  * searches, integer block SADs, sub-pel probes, search samples (SURVEY 8d: (n_int+1) w h + n_sub ((w+5)(h+5) + w h)), predictions, prediction samples,
  * transform chains, chain samples (3 N^2), intra predictions, intra samples (4N + N^2), SSD/SAD samples (2 w h), super blocks */

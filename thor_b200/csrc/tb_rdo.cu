@@ -443,8 +443,8 @@ constexpr int RDO_CTAS_PER_SM = 1;
 // One row of super blocks of one frame of the batch.  Rows are the unit a CTA claims; super blocks inside a row are sequential.
 // path = nsbx + 2 (nsby - 1 - row): super blocks on the longest dependency chain from the row's first super block to the end of its frame.
 struct RowDesc { int frame, row, nsbx, path; };
-// scheduler words behind the per-row arrays
-enum { CTL_REMAINING = 0, CTL_ERROR = 1, CTL_EVENT = 2 /* bumped after every finished super block */, CTL_N = 4 };
+// scheduler words behind the per-row arrays, zeroed before every launch
+enum { CTL_DONE = 0 /* super blocks finished */, CTL_ERROR = 1, CTL_EVENT = 2 /* bumped after every finished super block */, CTL_N = 4 };
 
 __device__ __forceinline__ unsigned long long globaltimer() {
   unsigned long long t;
@@ -463,7 +463,7 @@ __device__ __forceinline__ unsigned long long globaltimer() {
 // blocks is read through L2, see TB_LDF above).  Every finished super block is recorded in trace[] in completion order (tb_rdo_batch_trace).
 template <class S>
 __global__ void __launch_bounds__(32 * RDO_WARPS, RDO_CTAS_PER_SM)
-    rdo_batch_kernel(const FrameCtx<S> *ctxs, const RowDesc *rows, int nrows, Work<S> *works, int *prog, int *claimed, int *ctl, unsigned long long *prof_out,
+    rdo_batch_kernel(const FrameCtx<S> *ctxs, const RowDesc *rows, int nrows, int nsb, Work<S> *works, int *prog, int *claimed, int *ctl, unsigned long long *prof_out,
                      tb_rdo_sb_trace_t *trace) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   RdoCta &cta = *(RdoCta *)smem_raw;
@@ -509,7 +509,7 @@ __global__ void __launch_bounds__(32 * RDO_WARPS, RDO_CTAS_PER_SM)
           int f = 0;
           const int ev0 = cta.x_idx[1];
           while (true) {
-            if (vctl[CTL_REMAINING] <= 0) { f = 1; break; }
+            if (vctl[CTL_DONE] >= nsb) { f = 1; break; }
             // ~30 s of SM clocks without any work for this CTA while work remains: a row stopped publishing (it faulted): do not hang the launch
             if (vctl[CTL_ERROR] != 0 || clock64() - idle_since > 60000000000ll) { vctl[CTL_ERROR] = 1; f = 1; break; }
             if (vctl[CTL_EVENT] != ev0) break;
@@ -557,7 +557,7 @@ __global__ void __launch_bounds__(32 * RDO_WARPS, RDO_CTAS_PER_SM)
         const unsigned long long t_end = globaltimer();  // before the progress is published: a dependent super block starts after it
         sh.prof[ST_SB] += 1;
         vprog[sel] = sbx + 1;
-        atomicSub(&ctl[CTL_REMAINING], 1);
+        atomicAdd(&ctl[CTL_DONE], 1);
         __threadfence();
         atomicExch(&claimed[sel], 0);  // one super block per claim: the next claim re-chooses among all ready rows
         __threadfence();
@@ -604,15 +604,26 @@ struct Slot {
     blk = nullptr; leaves = nullptr; leaf_count = nullptr; coeffs = nullptr; w = 0; nref = 0; used = 0;
   }
 };
+// launches of a batch whose control words may be in flight at once: a further tb_rdo_batch_run waits for the oldest of them to finish
+constexpr int CTL_RING = 8;
 }  // namespace
 
+// Every call only enqueues, so the stream reads a pinned staging area (ctx_host, rows_host) and writes a read-back entry (ctl_host) after the call
+// has returned, possibly after later calls: each of them is rewritten on the host only once the event behind its last queued copy has completed,
+// and device buffers are freed only when the stream is idle.
 struct tb_rdo_batch {
   int nslots = 0, esz = 0, grid = 0, nrows = 0, nrows_cap = 0, grid_cap = 0;
   Slot *slots = nullptr;
-  void *ctx_host = nullptr, *ctx_dev = nullptr;  // FrameCtx<S>[nslots] (pinned staging, device copy)
+  void *ctx_host = nullptr, *ctx_dev = nullptr;  // FrameCtx<S>[nslots] (pinned staging, device copy); a slot's entry is copied by its upload
+  cudaEvent_t *ctx_ev = nullptr;                 // per slot: behind the copy of its ctx_host entry
   RowDesc *rows_host = nullptr, *rows_dev = nullptr;
+  cudaEvent_t rows_ev = nullptr;                 // behind the copy of rows_host
   int *sched_dev = nullptr;                      // prog[nrows] | claimed[nrows] | ctl[CTL_N]
-  int *ctl_host = nullptr;                       // pinned: ctl words read back after the launch
+  int *ctl_host = nullptr;                       // pinned: CTL_RING entries of CTL_N ctl words, read back after the launches in turn
+  cudaEvent_t ctl_ev[CTL_RING] = {};             // behind the read-back into each entry
+  int ctl_nsb[CTL_RING] = {};                    // super blocks of the launch an entry's words belong to; 0: no words pending
+  unsigned launches = 0;
+  int failed = 0, failed_left = 0;               // a launch since the last tb_rdo_batch_sync did not finish (failed_left super blocks left)
   void *works = nullptr;
   unsigned long long *prof = nullptr;
   tb_rdo_sb_trace_t *trace = nullptr;            // one entry per super block of the last launch, in completion order
@@ -627,7 +638,7 @@ template <class S> size_t smem_bytes() {
   return ((sizeof(RdoCta) + 15) & ~(size_t)15) + ((sizeof(FrameCtx<S>) + 15) & ~(size_t)15) + sizeof(RdoShared<S>) * RDO_WARPS;
 }
 
-int slot_prepare(Slot &D, const tb_rdo_frame_t *f) {
+int slot_prepare(Slot &D, const tb_rdo_frame_t *f, cudaStream_t st) {
   const int w = f->width, h = f->height, sb = 1 << f->log2_sb_size, esz = f->sample_bytes;
   // device planes use the padded geometry of the caller's reference frames; a frame without references (intra) may leave it unset:
   // then the reference's own geometry (common/common_frame.c:435-452 with PADDING_Y = 160)
@@ -635,6 +646,7 @@ int slot_prepare(Slot &D, const tb_rdo_frame_t *f) {
   const int sy = f->ref_stride[0] > 0 ? f->ref_stride[0] : ((w + 2 * pad + 15) & ~15), sc = f->ref_stride[0] > 0 ? f->ref_stride[1] : (((w >> 1) + 2 * padc + 15) & ~15);
   const size_t ref_y_bytes = (size_t)(h + 2 * pad) * sy * esz, ref_c_bytes = (size_t)((h >> 1) + 2 * padc) * sc * esz;
   if (D.w != w || D.h != h || D.esz != esz || D.sb != sb || D.pad != pad || D.sy != sy || D.sc != sc || D.nref < f->num_ref) {
+    if (D.w) CK(cudaStreamSynchronize(st));  // queued launches and downloads may still read the slot's buffers
     D.release();
     D.nsbx = (w + sb - 1) / sb; D.nsby = (h + sb - 1) / sb;
     const int nsb = D.nsbx * D.nsby;
@@ -682,10 +694,31 @@ int check_desc(const tb_rdo_frame_t *f) {
   return TB_OK;
 }
 
+// the control words a finished launch left in ctl_host entry k: a launch that did not finish every super block fails the next tb_rdo_batch_sync
+void collect_ctl(tb_rdo_batch *b, int k) {
+  const int *c = b->ctl_host + k * CTL_N;
+  if (c[CTL_ERROR] || c[CTL_DONE] != b->ctl_nsb[k]) { b->failed = 1; b->failed_left = b->ctl_nsb[k] - c[CTL_DONE]; }
+  b->ctl_nsb[k] = 0;
+}
+
 template <class S> int batch_launch(tb_rdo_batch *b, int n_active, cudaStream_t st) {
   // rows of the active slots, frame-major (the index breaks ties between rows of equal remaining path)
   int nrows = 0, nsb_total = 0;
   for (int s = 0; s < n_active; s++) { nrows += b->slots[s].nsby; nsb_total += b->slots[s].nsby * b->slots[s].nsbx; }
+  const size_t smem = smem_bytes<S>();
+  static bool attr_set[3] = {false, false, false};
+  static int per_sm[3] = {0, 0, 0};
+  if (!attr_set[sizeof(S)]) {
+    CK(cudaFuncSetAttribute(rdo_batch_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[sizeof(S)], rdo_batch_kernel<S>, 32 * RDO_WARPS, smem));
+    attr_set[sizeof(S)] = true;
+  }
+  if (!b->sms) { int dev = 0; CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&b->sms, cudaDevAttrMultiProcessorCount, dev)); }
+  // persistent grid: every CTA is resident (a CTA may spin until a neighbour publishes), never more CTAs than rows
+  int grid = b->sms * (per_sm[sizeof(S)] > 0 ? per_sm[sizeof(S)] : 1);
+  if (grid > nrows) grid = nrows;
+  // queued launches of this batch still use the buffers that grow here
+  if (b->launches && (nrows > b->nrows_cap || nsb_total > b->trace_cap || grid > b->grid_cap)) CK(cudaStreamSynchronize(st));
   if (nrows > b->nrows_cap) {
     cudaFreeHost(b->rows_host); cudaFree(b->rows_dev); cudaFree(b->sched_dev);
     b->rows_host = nullptr; b->rows_dev = nullptr; b->sched_dev = nullptr; b->nrows_cap = 0;
@@ -699,7 +732,13 @@ template <class S> int batch_launch(tb_rdo_batch *b, int n_active, cudaStream_t 
     CK(cudaMalloc((void **)&b->trace, sizeof(tb_rdo_sb_trace_t) * nsb_total));
     b->trace_cap = nsb_total;
   }
-  if (!b->ctl_host) CK(cudaMallocHost((void **)&b->ctl_host, sizeof(int) * CTL_N));
+  if (grid > b->grid_cap) {
+    cudaFree(b->works); b->works = nullptr; b->grid_cap = 0;
+    CK(cudaMalloc(&b->works, sizeof(Work<S>) * (size_t)grid * RDO_WARPS));
+    b->grid_cap = grid;
+  }
+  if (!b->prof) CK(cudaMalloc((void **)&b->prof, sizeof(unsigned long long) * ST_END));
+  CK(cudaEventSynchronize(b->rows_ev));  // the previous launch's row table has been copied
   int g = 0;
   for (int s = 0; s < n_active; s++) {
     const Slot &D = b->slots[s];
@@ -707,35 +746,24 @@ template <class S> int batch_launch(tb_rdo_batch *b, int n_active, cudaStream_t 
   }
   b->nrows = nrows;
   b->nsb = nsb_total;
-  const size_t smem = smem_bytes<S>();
-  static bool attr_set[3] = {false, false, false};
-  static int per_sm[3] = {0, 0, 0};
-  if (!attr_set[sizeof(S)]) {
-    CK(cudaFuncSetAttribute(rdo_batch_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm[sizeof(S)], rdo_batch_kernel<S>, 32 * RDO_WARPS, smem));
-    attr_set[sizeof(S)] = true;
-  }
-  if (!b->sms) { int dev = 0; CK(cudaGetDevice(&dev)); CK(cudaDeviceGetAttribute(&b->sms, cudaDevAttrMultiProcessorCount, dev)); }
-  // persistent grid: every CTA is resident (a CTA may spin until a neighbour publishes), never more CTAs than rows
-  int grid = b->sms * (per_sm[sizeof(S)] > 0 ? per_sm[sizeof(S)] : 1);
-  if (grid > nrows) grid = nrows;
-  if (grid > b->grid_cap) {
-    cudaFree(b->works); b->works = nullptr; b->grid_cap = 0;
-    CK(cudaMalloc(&b->works, sizeof(Work<S>) * (size_t)grid * RDO_WARPS));
-    b->grid_cap = grid;
-  }
   b->grid = grid;
-  if (!b->prof) CK(cudaMalloc((void **)&b->prof, sizeof(unsigned long long) * ST_END));
   CK(cudaMemcpyAsync(b->rows_dev, b->rows_host, sizeof(RowDesc) * nrows, cudaMemcpyDefault, st));
-  CK(cudaMemcpyAsync(b->ctx_dev, b->ctx_host, sizeof(FrameCtx<S>) * n_active, cudaMemcpyDefault, st));
+  CK(cudaEventRecord(b->rows_ev, st));
+  // the frame parameters were copied by the uploads; the scheduler words start at zero, the super-block count is an argument
   CK(cudaMemsetAsync(b->sched_dev, 0, sizeof(int) * (2 * (size_t)nrows + CTL_N), st));
-  b->ctl_host[CTL_REMAINING] = nsb_total; b->ctl_host[CTL_ERROR] = 0; b->ctl_host[2] = b->ctl_host[3] = 0;
-  CK(cudaMemcpyAsync(b->sched_dev + 2 * (size_t)nrows, b->ctl_host, sizeof(int) * CTL_N, cudaMemcpyDefault, st));
   CK(cudaMemsetAsync(b->prof, 0, sizeof(unsigned long long) * ST_END, st));
-  rdo_batch_kernel<S><<<grid, 32 * RDO_WARPS, smem, st>>>((const FrameCtx<S> *)b->ctx_dev, b->rows_dev, nrows, (Work<S> *)b->works, b->sched_dev, b->sched_dev + nrows,
-                                                         b->sched_dev + 2 * (size_t)nrows, b->prof, b->trace);
+  rdo_batch_kernel<S><<<grid, 32 * RDO_WARPS, smem, st>>>((const FrameCtx<S> *)b->ctx_dev, b->rows_dev, nrows, nsb_total, (Work<S> *)b->works, b->sched_dev,
+                                                         b->sched_dev + nrows, b->sched_dev + 2 * (size_t)nrows, b->prof, b->trace);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(b->ctl_host, b->sched_dev + 2 * (size_t)nrows, sizeof(int) * CTL_N, cudaMemcpyDefault, st));
+  // this launch's control words go to an entry of their own; the entry's previous launch (CTL_RING launches back) is checked first
+  const int k = (int)(b->launches++ % CTL_RING);
+  if (b->ctl_nsb[k]) {
+    CK(cudaEventSynchronize(b->ctl_ev[k]));
+    collect_ctl(b, k);
+  }
+  CK(cudaMemcpyAsync(b->ctl_host + k * CTL_N, b->sched_dev + 2 * (size_t)nrows, sizeof(int) * CTL_N, cudaMemcpyDefault, st));
+  CK(cudaEventRecord(b->ctl_ev[k], st));
+  b->ctl_nsb[k] = nsb_total;
   return TB_OK;
 }
 
@@ -752,8 +780,14 @@ tb_rdo_batch_t *tb_rdo_batch_create(int n_slots, int sample_bytes) {
   tb_rdo_batch *b = new tb_rdo_batch();
   b->nslots = n_slots; b->esz = sample_bytes;
   b->slots = new Slot[n_slots];
+  b->ctx_ev = new cudaEvent_t[n_slots]();
   const size_t cb = (sample_bytes == 1 ? sizeof(FrameCtx<uint8_t>) : sizeof(FrameCtx<uint16_t>)) * (size_t)n_slots;
-  if (cudaMallocHost(&b->ctx_host, cb) != cudaSuccess || cudaMalloc(&b->ctx_dev, cb) != cudaSuccess) {
+  bool ok = cudaMallocHost(&b->ctx_host, cb) == cudaSuccess && cudaMalloc(&b->ctx_dev, cb) == cudaSuccess &&
+            cudaMallocHost((void **)&b->ctl_host, sizeof(int) * CTL_RING * CTL_N) == cudaSuccess &&
+            cudaEventCreateWithFlags(&b->rows_ev, cudaEventDisableTiming) == cudaSuccess;
+  for (int s = 0; ok && s < n_slots; s++) ok = cudaEventCreateWithFlags(&b->ctx_ev[s], cudaEventDisableTiming) == cudaSuccess;
+  for (int k = 0; ok && k < CTL_RING; k++) ok = cudaEventCreateWithFlags(&b->ctl_ev[k], cudaEventDisableTiming) == cudaSuccess;
+  if (!ok) {
     snprintf(g_err, sizeof(g_err), "tb_rdo_batch_create: out of memory");
     tb_rdo_batch_destroy(b);
     return nullptr;
@@ -768,6 +802,12 @@ void tb_rdo_batch_destroy(tb_rdo_batch_t *b) {
   delete[] b->slots;
   cudaFreeHost(b->ctx_host); cudaFree(b->ctx_dev); cudaFreeHost(b->rows_host); cudaFree(b->rows_dev); cudaFree(b->sched_dev); cudaFreeHost(b->ctl_host);
   cudaFree(b->works); cudaFree(b->prof); cudaFree(b->trace);
+  for (int s = 0; s < b->nslots; s++)
+    if (b->ctx_ev[s]) cudaEventDestroy(b->ctx_ev[s]);
+  delete[] b->ctx_ev;
+  if (b->rows_ev) cudaEventDestroy(b->rows_ev);
+  for (int k = 0; k < CTL_RING; k++)
+    if (b->ctl_ev[k]) cudaEventDestroy(b->ctl_ev[k]);
   delete b;
 }
 
@@ -777,12 +817,17 @@ int tb_rdo_batch_upload(tb_rdo_batch_t *b, int slot, const tb_rdo_frame_t *f) {
   if (f->sample_bytes != b->esz) { snprintf(g_err, sizeof(g_err), "tb_rdo_batch_upload: sample size differs from the batch's"); return TB_ERR_ARG; }
   cudaStream_t st = (cudaStream_t)tb_stream();
   Slot &D = b->slots[slot];
-  if (slot_prepare(D, f) != TB_OK) return TB_ERR_CUDA;
+  if (slot_prepare(D, f, st) != TB_OK) return TB_ERR_CUDA;
   const int esz = D.esz, w = D.w, h = D.h, padc = D.pad >> 1;
   const size_t oy = ((size_t)D.pad * D.sy + D.pad) * esz, oc = ((size_t)padc * D.sc + padc) * esz;
   const size_t ref_y_bytes = (size_t)(h + 2 * D.pad) * D.sy * esz, ref_c_bytes = (size_t)((h >> 1) + 2 * padc) * D.sc * esz;
+  // frame parameters: the slot's staging entry is rewritten once the copy of its previous upload has run
+  const size_t csz = esz == 1 ? sizeof(FrameCtx<uint8_t>) : sizeof(FrameCtx<uint16_t>);
+  CK(cudaEventSynchronize(b->ctx_ev[slot]));
   if (esz == 1) fill_ctx(((FrameCtx<uint8_t> *)b->ctx_host)[slot], D, f);
   else fill_ctx(((FrameCtx<uint16_t> *)b->ctx_host)[slot], D, f);
+  CK(cudaMemcpyAsync((char *)b->ctx_dev + slot * csz, (const char *)b->ctx_host + slot * csz, csz, cudaMemcpyDefault, st));
+  CK(cudaEventRecord(b->ctx_ev[slot], st));
   // uploads: source (visible area), references (whole padded planes: one contiguous copy each)
   for (int p = 0; p < 3; p++)
     CK(cudaMemcpy2DAsync((char *)D.org[p] + (p ? oc : oy), (size_t)(p ? D.sc : D.sy) * esz, f->orig[p], (size_t)f->orig_stride[p ? 1 : 0] * esz, (size_t)(p ? w >> 1 : w) * esz,
@@ -861,8 +906,11 @@ int tb_rdo_batch_sync(tb_rdo_batch_t *b) {
     for (int k = 0; k < 6; k++) fprintf(stderr, " %.1f%%", 100.0 * (double)pr[ST_IP_SZ + k] / (double)(pr[PF_INTERP] ? pr[PF_INTERP] : 1));
     fprintf(stderr, "\n");
   }
-  if (b->ctl_host && (b->ctl_host[CTL_ERROR] || b->ctl_host[CTL_REMAINING] != 0)) {
-    snprintf(g_err, sizeof(g_err), "rdo_batch_kernel: a super-block row stopped publishing progress (%d super blocks left)", b->ctl_host[CTL_REMAINING]);
+  for (int k = 0; k < CTL_RING; k++)
+    if (b->ctl_nsb[k]) collect_ctl(b, k);
+  if (b->failed) {
+    snprintf(g_err, sizeof(g_err), "rdo_batch_kernel: a super-block row stopped publishing progress (%d super blocks left)", b->failed_left);
+    b->failed = 0;
     return TB_ERR_CUDA;
   }
   return TB_OK;
