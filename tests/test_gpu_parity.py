@@ -316,21 +316,10 @@ def test_batch_sad(tb, hbd, bd):
                 assert got64[i] == getattr(O, "orc_ssd_" + s)(a, b, cur.sy, href.sy, bw, bh), i
 
 
-def me_form(bw, bh, speed, esz):
-    """the search form a batch gives an item, restated from MeClassOf / me_class (tb_kernels.cuh): the whole CTA for speed 0 and >= 2048
-    samples in a multiple of 32 rows, four per warp for 8-bit speed-0 blocks of <= 64 samples in multiples of 4, one warp otherwise"""
-    if speed == 0 and bw * bh >= 2048 and bh % 32 == 0:
-        return "team"
-    if esz == 1 and speed == 0 and bw * bh <= 64 and not (bw | bh) & 3:
-        return "quad"
-    return "warp"
-
-
 def me_batch(tb, rng, hbd, bd, w, h, n, edge, sizes, speed, bip):
     """n searches on a w x h frame pair in one tb_motion_estimate_batch, the last `edge` of them placed at the picture's edges (edge_search,
-    signs alternating; their blocks come from a buffer of their own), each against the oracle.  Returns (differences, reach, forms):
-    reach[sign] counts the edge results on a clip_mv limit / through an active split_mv clamp (edge_reach), forms the search forms the edge
-    items were given."""
+    signs alternating; their blocks come from a buffer of their own), each against the oracle.  Returns (differences, reach):
+    reach[sign] counts the edge results on a clip_mv limit / through an active split_mv clamp (edge_reach)."""
     s = sfx(hbd)
     esz = 2 if hbd else 1
     href, cur, dref, dcur, _ = make_frames(tb, rng, w, h, bd, hbd)
@@ -373,7 +362,7 @@ def me_batch(tb, rng, hbd, bd, w, h, n, edge, sizes, speed, bip):
     d_items = tb.DevBuf.from_array(items); d_c = tb.DevBuf.from_array(call); d_out = tb.DevBuf(8 * n)
     tb.check(tb.lib.tb_motion_estimate_batch(d_items.ptr, n, d_c.ptr, esz, bd, speed, bip, w, h, d_out.ptr))
     got = d_out.download(tb.ME_RESULT, n)
-    bad, reach, forms = [], np.zeros((2, 2), int), {True: set(), False: set()}
+    bad, reach = [], np.zeros((2, 2), int)
     for i, (blk, is_edge, size, bw, bh, ox, oy, xpos, ypos, sign, cc, mvc, mvp, lam) in enumerate(meta):
         org = aligned((size, size), sdt(hbd))
         org[...] = blk
@@ -385,21 +374,19 @@ def me_batch(tb, rng, hbd, bd, w, h, n, edge, sizes, speed, bip):
         res = (int(got[i]["cost"]), int(got[i]["mvx"]), int(got[i]["mvy"]))
         if res != (cost & 0xffffffff, m0[0], m0[1]):
             bad.append((w, h, i, is_edge, size, bw, bh, xpos, ypos, sign, len(cc), res, (cost, m0[0], m0[1])))
-        forms[is_edge].add(me_form(bw, bh, speed, esz))
         if is_edge:
             reach[sign] += edge_reach(res[1], res[2], sign, xpos, ypos, w, h, size, bw, bh)
-    assert not edge or forms[True] == forms[False], forms  # every search form the batch uses gets edge items
-    return bad, reach, forms[True]
+    return bad, reach
 
 
 def me_batches(tb, hbd, bd, seed, dims, n, edge, sizes, speed, bip):
-    """me_batch on each frame size of dims; the differences, reach and forms of all of them"""
+    """me_batch on each frame size of dims; the differences and reach of all of them"""
     rng = np.random.default_rng(seed)
-    bad, reach, forms = [], np.zeros((2, 2), int), set()
+    bad, reach = [], np.zeros((2, 2), int)
     for w, h in dims:
-        b, r, f = me_batch(tb, rng, hbd, bd, w, h, n, edge, sizes, speed, bip)
-        bad += b; reach += r; forms |= f
-    return bad, reach, forms
+        b, r = me_batch(tb, rng, hbd, bd, w, h, n, edge, sizes, speed, bip)
+        bad += b; reach += r
+    return bad, reach
 
 
 # the edge searches' results per sign on a clip_mv limit / through an active split_mv clamp, at least, as fractions of the edge items of one
@@ -412,30 +399,26 @@ EDGE_DIMS = ((256, 192), (200, 136))
 @pytest.mark.parametrize("hbd,bd", BD)
 @pytest.mark.parametrize("speed,bip", [(0, 1), (0, 0), (1, 0), (2, 0), (1, 1)])
 def test_batch_motion_estimate(tb, hbd, bd, speed, bip):
-    """every search form (one warp, four per warp, the CTA team) at random positions and at the picture's edges"""
-    bad, reach, forms = me_batches(tb, hbd, bd, 108 + speed * 7 + bip, EDGE_DIMS, 160, 64, (8, 16, 32, 64), speed, bip)
+    """8x8 .. 64x64 coding blocks and their partitions at random positions and at the picture's edges; same results as the oracle"""
+    bad, reach = me_batches(tb, hbd, bd, 108 + speed * 7 + bip, EDGE_DIMS, 160, 64, (8, 16, 32, 64), speed, bip)
     assert not bad, (len(bad), bad[:8])
-    assert forms == ({"warp", "team", "quad"} if speed == 0 and not hbd else {"warp", "team"} if speed == 0 else {"warp"}), forms
     assert (reach >= ME_EDGE_REACH * 64).all(), reach
 
 
 @pytest.mark.parametrize("hbd,bd", BD)
 @pytest.mark.parametrize("sizes,n,bip", [((8,), 160, 1), ((8, 16), 480, 1), ((8,), 96, 0)])
 def test_motion_estimate_small_blocks(tb, hbd, bd, sizes, n, bip):
-    """blocks of <= 64 samples: four searches share a warp on 8-bit frames (quad_motion_estimate), incl. the wide-SAD candidates of
-    8x8 partitions of 16x16 coding blocks; same results as the oracle"""
-    bad, reach, forms = me_batches(tb, hbd, bd, 137 + n, EDGE_DIMS, n, n // 2, sizes, 0, bip)
+    """blocks of <= 64 samples, incl. the wide-SAD candidates of 8x8 partitions of 16x16 coding blocks; same results as the oracle"""
+    bad, reach = me_batches(tb, hbd, bd, 137 + n, EDGE_DIMS, n, n // 2, sizes, 0, bip)
     assert not bad, (len(bad), bad[:6])
-    assert ("quad" in forms) == (not hbd), forms
     assert (reach >= ME_EDGE_REACH * (n // 2)).all(), reach
 
 
 @pytest.mark.parametrize("hbd,bd", BD)
 def test_motion_estimate_large_blocks(tb, hbd, bd):
-    """64x64 .. 128x128 prediction blocks are searched by a whole CTA (four warps on row bands); same results as the oracle"""
-    bad, reach, forms = me_batches(tb, hbd, bd, 131, ((384, 256), (200, 136)), 36, 18, (64, 128), 0, 1)
+    """64x64 and 128x128 coding blocks and their partitions (32x32 .. 128x128 prediction blocks); same results as the oracle"""
+    bad, reach = me_batches(tb, hbd, bd, 131, ((384, 256), (200, 136)), 36, 18, (64, 128), 0, 1)
     assert not bad, (len(bad), bad[:6])
-    assert forms == {"warp", "team"}, forms
     assert (reach >= ME_EDGE_REACH * 18).all(), reach
 
 

@@ -50,13 +50,6 @@ bool ensure_ctx() {
   if (cudaGetDeviceProperties(&prop, dev) == cudaSuccess) g.sm_count = prop.multiProcessorCount;
   if ((e = cudaStreamCreateWithFlags(&g.stream, cudaStreamNonBlocking)) != cudaSuccess) { set_err("cudaStreamCreate", e); g.failed = true; return false; }
   g.own_stream = true;
-  {  // stream-ordered scratch (cudaMallocAsync) stays cached in the pool across synchronisations instead of going back to the driver
-    cudaMemPool_t pool;
-    if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-      uint64_t keep = ~0ull;
-      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-    }
-  }
   g.ready = true;
   return true;
 }
@@ -70,12 +63,6 @@ inline void need_ctx(const char *where) {
 inline void ck(cudaError_t e, const char *where) {
   if (e != cudaSuccess) { set_err(where, e); die(where); }
 }
-// the batched (B) entry points promise TB_ERR_CUDA, not abort(): only the drop-in symbols (no error channel in the reference's ABI) die
-#define CKB(x, where)                                                        \
-  do {                                                                       \
-    cudaError_t e__ = (x);                                                   \
-    if (e__ != cudaSuccess) { set_err(where, e__); return TB_ERR_CUDA; }     \
-  } while (0)
 void *slot_buf(int s, size_t bytes) {
   if (g.cap[s] < bytes) {
     if (g.slot[s]) { ck(cudaStreamSynchronize(g.stream), "sync"); cudaFree(g.slot[s]); }
@@ -395,20 +382,8 @@ int tb_motion_estimate_batch(const tb_me_item_t *items, int n, const int16_t *ca
   API_BEGIN();
   if (sample_bytes != 1 && sample_bytes != 2) { set_err("tb_motion_estimate_batch: sample_bytes must be 1 or 2", cudaSuccess); return TB_ERR_ARG; }
   if (n <= 0) return TB_OK;
-  // stream-ordered scratch: the sorted item list and the scheduler's counters (see me_batch_kernel)
-  int *meta = nullptr, *idx = nullptr;
-  CKB(cudaMallocAsync((void **)&meta, 128 * sizeof(int) + (size_t)n * sizeof(int), g.stream), "me scratch");
-  idx = meta + 128;
-  CKB(cudaMemsetAsync(meta, 0, 128 * sizeof(int), g.stream), "me scratch");
-  const int sgrid = std::min((n + 255) / 256, g.sm_count * 8);
-  const MeClassOf cls{speed, (sample_bytes == 1 && speed == 0) ? 1 : 0};
-  LAUNCH((sched_hist_kernel<tb_me_item_t, MeClassOf>), sgrid, 256, 0, items, n, cls, meta);
-  LAUNCH(sched_scan_kernel, 1, 32, 0, meta);
-  LAUNCH((sched_scatter_kernel<tb_me_item_t, MeClassOf>), sgrid, 256, 0, items, n, cls, meta, idx);
-  const int grid = std::min((n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, g.sm_count * ME_MINBLOCKS);  // persistent: every CTA resident
-  if (sample_bytes == 1) LAUNCH(me_batch_kernel<uint8_t>, grid, CTA_THREADS, 0, items, n, idx, meta, cand, bitdepth, speed, bip, fw, fh, out, g.me_stats);
-  else LAUNCH(me_batch_kernel<uint16_t>, grid, CTA_THREADS, 0, items, n, idx, meta, cand, bitdepth, speed, bip, fw, fh, out, g.me_stats);
-  CKB(cudaFreeAsync(meta, g.stream), "me scratch");
+  if (sample_bytes == 1) LAUNCH(me_batch_kernel<uint8_t>, grid_for_warps(n), CTA_THREADS, 0, items, n, cand, bitdepth, speed, bip, fw, fh, out, g.me_stats);
+  else LAUNCH(me_batch_kernel<uint16_t>, grid_for_warps(n), CTA_THREADS, 0, items, n, cand, bitdepth, speed, bip, fw, fh, out, g.me_stats);
   API_END();
 }
 int tb_motion_estimate_bi_batch(const tb_me_bi_item_t *items, int n, const int16_t *cand, int sample_bytes, int bitdepth, int bip, int fw, int fh, tb_me_result_t *out) {

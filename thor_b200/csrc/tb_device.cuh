@@ -16,9 +16,6 @@
 // TB_LDG: read-only-path load of data that no thread writes during the kernel (frames, work items).  TB_LDF: load of reconstructed
 // samples that ANOTHER CTA may have written earlier in the same kernel (wavefront RD loop, tb_rdo.cu): that translation unit maps
 // TB_LDG to a plain load (its "original" block can be a scratch block written moments ago) and TB_LDF to an L1-bypassing load.
-#ifndef TB_SAD_ROWS
-#define TB_SAD_ROWS 0
-#endif
 #ifndef TB_ROLL
 #define TB_ROLL  // tb_rdo.cu: "#pragma unroll 1" on the simple per-sample loops (its kernel is bound by instruction fetch)
 #endif
@@ -36,7 +33,7 @@ namespace tb {
 
 constexpr unsigned FULL = 0xffffffffu;
 constexpr int TX_MINBLOCKS = 5;  // __launch_bounds__(128, N) of the transform-chain kernel: registers/thread <= 65536 / (128 N); its shared memory allows 5
-constexpr int ME_MINBLOCKS = 6;  // __launch_bounds__(128, N) of the motion-search kernel: registers/thread <= 65536 / (128 N)
+constexpr int ME_MINBLOCKS = 4;  // __launch_bounds__(128, N) of the motion-search kernel: registers/thread <= 65536 / (128 N); with fewer than 128 it spills
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ int ilog2(int x) { return 31 - __clz(x); }                       // common/simd.h:86
@@ -79,30 +76,7 @@ template <class S> __device__ __forceinline__ uint32_t word_sad(uint32_t a, uint
 // `o` must be 4-byte aligned with an even word pitch (original blocks always are); `r` arbitrary.
 // Lanes sub..sub+nl-1 of a group share the block; returns this lane's partial sum.
 // ---------------------------------------------------------------------------------------------------------------
-// Rows of >= 16 bytes with 128-bit loads: one aligned LDG.128 per 16 reference bytes (+1 per row) and one per 16 original
-// bytes instead of eight 32-bit loads — the search is designed for L1 wavefronts as its bound, so
-// request count matters more than bytes.  J = word offset of the row inside its first 16-byte chunk (uniform per lane group:
-// all pitches are multiples of 16 bytes), sh = remaining byte offset in bits.
-template <class S, int J>
-__device__ __forceinline__ uint32_t sad_rows_v4(const uint4 *rq, int rsv, const uint4 *oq, int osv, int nch, int h, int sub, int nl, unsigned sh) {
-  uint32_t acc = 0;
-  for (int row = sub; row < h; row += nl) {
-    const uint4 *q = rq + row * rsv, *a = oq + row * osv;
-    uint4 P = TB_LDG(q);
-    for (int c = 0; c < nch; c++) {
-      const uint4 N = TB_LDG(q + c + 1), A = TB_LDG(a + c);
-      const uint32_t w0 = J == 0 ? P.x : (J == 1 ? P.y : (J == 2 ? P.z : P.w)), w1 = J == 0 ? P.y : (J == 1 ? P.z : (J == 2 ? P.w : N.x)),
-                     w2 = J == 0 ? P.z : (J == 1 ? P.w : (J == 2 ? N.x : N.y)), w3 = J == 0 ? P.w : (J == 1 ? N.x : (J == 2 ? N.y : N.z)),
-                     w4 = J == 0 ? N.x : (J == 1 ? N.y : (J == 2 ? N.z : N.w));
-      acc += word_sad<S>(A.x, __funnelshift_r(w0, w1, sh)) + word_sad<S>(A.y, __funnelshift_r(w1, w2, sh)) + word_sad<S>(A.z, __funnelshift_r(w2, w3, sh)) +
-             word_sad<S>(A.w, __funnelshift_r(w3, w4, sh));
-      P = N;
-    }
-  }
-  return acc;
-}
-
-template <class S, bool V4 = false>
+template <class S>
 __device__ __forceinline__ uint32_t sad_partial(const S *o, int os, const S *r, int rs, int w, int h, int sub, int nl) {
   // Lane `sub` of `nl` takes the rows sub, sub+nl, ... (nl <= h).  Row pitches are multiples of 4 bytes, so the byte
   // misalignment of the reference row is the same for every row: one aligned word stream per row, one funnel shift per word.
@@ -113,16 +87,6 @@ __device__ __forceinline__ uint32_t sad_partial(const S *o, int os, const S *r, 
   const uint32_t *rq = (const uint32_t *)(ra & ~(uintptr_t)3);
   const uint32_t *oq = (const uint32_t *)o;
   const int rsw = (rs * (int)sizeof(S)) >> 2, osw = (os * (int)sizeof(S)) >> 2;  // pitches in words
-  if (V4 && !(ww & 3) && !((((uintptr_t)o) | (unsigned)(osw << 2) | (unsigned)(rsw << 2)) & 15)) {
-    const uint4 *rv = (const uint4 *)(ra & ~(uintptr_t)15), *ov = (const uint4 *)o;
-    const unsigned sh8 = (unsigned)(ra & 3) * 8;
-    switch ((unsigned)(ra >> 2) & 3) {
-      case 0: return sad_rows_v4<S, 0>(rv, rsw >> 2, ov, osw >> 2, ww >> 2, h, sub, nl, sh8);
-      case 1: return sad_rows_v4<S, 1>(rv, rsw >> 2, ov, osw >> 2, ww >> 2, h, sub, nl, sh8);
-      case 2: return sad_rows_v4<S, 2>(rv, rsw >> 2, ov, osw >> 2, ww >> 2, h, sub, nl, sh8);
-      default: return sad_rows_v4<S, 3>(rv, rsw >> 2, ov, osw >> 2, ww >> 2, h, sub, nl, sh8);
-    }
-  }
   uint32_t acc = 0;
   TB_ROLL
   for (int row = sub; row < h; row += nl) {
@@ -178,37 +142,7 @@ __device__ __noinline__ uint32_t multi_sad_narrow(const S *o, int os, const S *r
   return out;
 }
 
-// The same for blocks of >= 256 words whose rows are >= 16 bytes: 16 or 32 lanes per position, so at most two positions (two
-// chunk offsets) are in flight per pass and the 128-bit row loads of sad_rows_v4 stay (nearly) uniform.  A separate function:
-// its larger register footprint must not be paid around the calls for small blocks.
-template <class S>
-__device__ __noinline__ uint32_t multi_sad_wide(const S *o, int os, const S *r, int rs, int w, int h, int roff, int n) {
-  constexpr int PW = Word<S>::PW;
-  const int lane = lane_id();
-  const int nwords = (w / PW) * h;
-  int L = nwords >= 512 ? 32 : 16;
-  if (L > h) L = h;  // h >= 16 here
-  uint32_t out = 0;
-  if (L == 32) {
-    for (int p = 0; p < n; p++) {
-      int off = __shfl_sync(FULL, roff, p);
-      uint32_t s = warp_sum(lane < h ? sad_partial<S, true>(o, os, r + off, rs, w, h, lane, 32) : 0u);
-      if (lane == p) out = s;
-    }
-  } else {
-    const int sub = lane & 15, grp = lane >> 4;
-    for (int base = 0; base < n; base += 2) {
-      int p = base + grp;
-      int off = __shfl_sync(FULL, roff, p & 31);
-      uint32_t s = (p < n) ? sad_partial<S, true>(o, os, r + off, rs, w, h, sub, 16) : 0u;
-      s = group_sum(s, 16);
-      uint32_t got = __shfl_sync(FULL, s, ((lane - base) * 16) & 31);
-      if (lane >= base && lane < base + 2 && lane < n) out = got;
-    }
-  }
-  return out;
-}
-// The same for the device-resident RD loop (tb_rdo.cu, TB_SAD_ROWS), where ONE warp walks blocks of up to 128x128 alone and nothing else hides its latency:
+// The same for rows of >= 8 words, where ONE warp walks blocks of up to 128x128 alone and nothing else hides its latency:
 // the lanes of a load request lie along a ROW (32-byte .. 128-byte contiguous segments: one or two L1 wavefronts per request instead of one per lane when
 // the rows are dealt to lanes), five positions share each load of the original (a telescope grid row: their reference segments overlap), and the five
 // accumulations are independent.  Rows >= 8 words; lane = (row % RP) * LW + word, RP rows per pass.
@@ -254,15 +188,9 @@ __device__ __noinline__ uint32_t multi_sad_rows(const S *o, int os, const S *r, 
   }
   return out;
 }
-template <class S, int TW = 1>
+template <class S>
 __device__ __forceinline__ uint32_t multi_sad(const S *o, int os, const S *r, int rs, int w, int h, int roff, int n) {
-  // only the CTA-team searches (blocks >= 2048 samples) take the wide form: a second callee at the call sites of the one-warp
-  // searches costs them more in spills than the 32x32 blocks would gain
-  if (TW > 1 && (w / Word<S>::PW) * h >= 256 && h >= 16 && w * (int)sizeof(S) >= 16) return multi_sad_wide<S>(o, os, r, rs, w, h, roff, n);
-#if TB_SAD_ROWS
-  if (TW == 1 && w / Word<S>::PW >= 8) return multi_sad_rows<S>(o, os, r, rs, w, h, roff, n);
-#endif
-  return multi_sad_narrow<S>(o, os, r, rs, w, h, roff, n);
+  return w / Word<S>::PW >= 8 ? multi_sad_rows<S>(o, os, r, rs, w, h, roff, n) : multi_sad_narrow<S>(o, os, r, rs, w, h, roff, n);
 }
 
 // a3: SSD.  enc/encode_block.c:455-465
@@ -525,13 +453,11 @@ __device__ __noinline__ void warp_interp_strips_u8(uint8_t *dst, int ds, const u
 // enc/encode_block.c:625-663) without materialising the predictions: probe t = lane / 4 uses MV (mvx0 + dx[t], mvy0 + dy[t]),
 // its four lanes share the block's samples.  Every lane of probe t returns SAD t.
 template <class S>
-__device__ __noinline__ uint32_t subpel_stage_sads(const S *o, int os, const S *ref, int rs, int w, int hfull, int mvx, int mvy, int sign, int bip, int pic_w, int pic_h,
-                                      int xpos, int ypos, int bitdepth, int row0, int h) {
-  // rows [row0, row0 + h) of the w x hfull block (a team of warps splits the block into row bands; one warp: row0 = 0, h = hfull)
+__device__ __noinline__ uint32_t subpel_stage_sads(const S *o, int os, const S *ref, int rs, int w, int h, int mvx, int mvy, int sign, int bip, int pic_w, int pic_h,
+                                      int xpos, int ypos, int bitdepth) {
   int hi, vi, xf, yf;
-  split_mv(mvx, mvy, sign, 2, pic_w, pic_h, xpos, ypos, w, hfull, hi, vi, xf, yf);
-  const S *ip = ref + (vi + row0) * rs + hi;
-  o += row0 * os;
+  split_mv(mvx, mvy, sign, 2, pic_w, pic_h, xpos, ypos, w, h, hi, vi, xf, yf);
+  const S *ip = ref + vi * rs + hi;
   const int maxv = (1 << bitdepth) - 1, lw = ilog2(w), sub = lane_id() & 3;
   uint32_t acc = 0;
   if (sizeof(S) == 1) {
@@ -571,12 +497,12 @@ __device__ __forceinline__ void row12_u8(const uint8_t *p, uint32_t &b0, uint32_
   const uint32_t w0 = TB_LDG(w), w1 = TB_LDG(w + 1), w2 = TB_LDG(w + 2), w3 = TB_LDG(w + 3);
   b0 = __funnelshift_r(w0, w1, sh); b1 = __funnelshift_r(w1, w2, sh); b2 = __funnelshift_r(w2, w3, sh);
 }
-__device__ __noinline__ uint32_t halfpel_stage_sads_u8(const uint8_t *o, int os, const uint8_t *ref, int rs, int w, int hfull, int bx, int by, const int8_t *dxs,
-                                                       const int8_t *dys, int sign, int bip, int pic_w, int pic_h, int xpos, int ypos, int row0, int h) {
+__device__ __noinline__ uint32_t halfpel_stage_sads_u8(const uint8_t *o, int os, const uint8_t *ref, int rs, int w, int h, int bx, int by, const int8_t *dxs,
+                                                       const int8_t *dys, int sign, int bip, int pic_w, int pic_h, int xpos, int ypos) {
   const int lane = lane_id(), t = lane & 7;
   const int mvx = (int)(int16_t)(bx + dxs[t + 1]), mvy = (int)(int16_t)(by + dys[t + 1]);
   int hi, vi, xf, yf;
-  split_mv(mvx, mvy, sign, 2, pic_w, pic_h, xpos, ypos, w, hfull, hi, vi, xf, yf);
+  split_mv(mvx, mvy, sign, 2, pic_w, pic_h, xpos, ypos, w, h, hi, vi, xf, yf);
   const int hmin = __reduce_min_sync(FULL, hi), vmin = __reduce_min_sync(FULL, vi);
   const int ho = hi - hmin, vo = vi - vmin;
   const int cls = (xf == 2 && yf == 0) ? 0 : ((xf == 0 && yf == 2) ? 1 : ((xf == 2 && yf == 2) ? 2 : 3));
@@ -587,8 +513,7 @@ __device__ __noinline__ uint32_t halfpel_stage_sads_u8(const uint8_t *o, int os,
   const int8_t *fh = c_luma_taps[bip ? 1 : 0][2];
   const uint32_t tlo = pack_s8x4(fh[0], fh[1], fh[2], fh[3]), thi = pack_s8x4(fh[4], fh[5], 0, 0);
   const int ns = w >> 2, lns = ilog2(ns);
-  const uint8_t *rb = ref + (row0 + vmin) * rs + hmin;  // plane sample (r, c) <-> rb[r * rs + c]
-  const uint8_t *ob = o + row0 * os;
+  const uint8_t *rb = ref + vmin * rs + hmin;  // plane sample (r, c) <-> rb[r * rs + c]
   uint32_t aH0 = 0, aH1 = 0, aV0 = 0, aV1 = 0, aC00 = 0, aC01 = 0, aC10 = 0, aC11 = 0;  // aC<vo><ho>
   // ---- H pass: block rows y (plane rows y + voH), plane columns 4 s .. 4 s + 4
   if (mH) {
@@ -602,7 +527,7 @@ __device__ __noinline__ uint32_t halfpel_stage_sads_u8(const uint8_t *o, int os,
         const uint32_t lo = k < 4 ? __funnelshift_r(b0, b1, 8 * k) : b1, hi4 = k < 4 ? __funnelshift_r(b1, b2, 8 * k) : b2;
         v[k] = (dp4a_us(lo, tlo, dp4a_us(hi4, thi, 32))) >> 6;
       }
-      const uint32_t ow = TB_LDG((const uint32_t *)(ob + y * os + 4 * st));
+      const uint32_t ow = TB_LDG((const uint32_t *)(o + y * os + 4 * st));
       aH0 += __vsadu4(ow, pack_sat_u8x4(v[0], v[1], v[2], v[3]));
       aH1 += __vsadu4(ow, pack_sat_u8x4(v[1], v[2], v[3], v[4]));
     }
@@ -627,8 +552,8 @@ __device__ __noinline__ uint32_t halfpel_stage_sads_u8(const uint8_t *o, int os,
         v[k] = dp4a_us(__byte_perm(t01, t23, 0x5410), tlo, dp4a_us(t45, thi, 32)) >> 6;  // thi has zero taps on the two upper bytes
       }
       const uint32_t pk = pack_sat_u8x4(v[0], v[1], v[2], v[3]);
-      if (r < h) aV0 += __vsadu4(TB_LDG((const uint32_t *)(ob + r * os + 4 * st)), pk);
-      if (r > 0) aV1 += __vsadu4(TB_LDG((const uint32_t *)(ob + (r - 1) * os + 4 * st)), pk);
+      if (r < h) aV0 += __vsadu4(TB_LDG((const uint32_t *)(o + r * os + 4 * st)), pk);
+      if (r > 0) aV1 += __vsadu4(TB_LDG((const uint32_t *)(o + (r - 1) * os + 4 * st)), pk);
     }
   }
   // ---- C pass: plane rows r = 0 .. h, plane columns 4 s .. 4 s + 4
@@ -656,12 +581,12 @@ __device__ __noinline__ uint32_t halfpel_stage_sads_u8(const uint8_t *o, int os,
       const uint32_t q0 = (uint32_t)(acc[0] >> 4), q1 = (uint32_t)(acc[1] >> 4), q2 = (uint32_t)(acc[2] >> 4), q3 = (uint32_t)(acc[3] >> 4), q4 = (uint32_t)(acc[4] >> 4);
       const uint32_t pk0 = q0 | (q1 << 8) | (q2 << 16) | (q3 << 24), pk1 = q1 | (q2 << 8) | (q3 << 16) | (q4 << 24);
       if (r < h) {
-        const uint32_t ow = TB_LDG((const uint32_t *)(ob + r * os + 4 * st));
+        const uint32_t ow = TB_LDG((const uint32_t *)(o + r * os + 4 * st));
         aC00 += __vsadu4(ow, pk0);
         aC01 += __vsadu4(ow, pk1);
       }
       if (r > 0) {
-        const uint32_t ow = TB_LDG((const uint32_t *)(ob + (r - 1) * os + 4 * st));
+        const uint32_t ow = TB_LDG((const uint32_t *)(o + (r - 1) * os + 4 * st));
         aC10 += __vsadu4(ow, pk0);
         aC11 += __vsadu4(ow, pk1);
       }
@@ -808,31 +733,10 @@ __device__ __forceinline__ int warp_first_min(uint32_t cost, int n, uint32_t &be
   return who ? __ffs(who) - 1 : -1;
 }
 
-// A team of TW warps (TW == 1, or the whole CTA) runs one search: every warp executes the same control flow on the same
-// totals and evaluates the SADs of its own band of h / TW rows; MeTeam::sum adds the per-lane partial SADs of the bands through
-// shared memory (two alternating buffers, one __syncthreads per exchange).
-template <int TW> struct MeTeam {
-  uint32_t *xch;  // [2][TW][32]
-  int warp, phase;
-  __device__ __forceinline__ uint32_t sum(uint32_t v) {
-    if (TW == 1) return v;
-    uint32_t *b = xch + (phase & 1) * TW * 32;
-    phase++;
-    b[warp * 32 + lane_id()] = v;
-    __syncthreads();
-    uint32_t t = 0;
-#pragma unroll
-    for (int k = 0; k < TW; k++) t += b[k * 32 + lane_id()];
-    return t;
-  }
-};
-
-template <class S, int TW>
-__device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_full, int rs, MeCtx &c, int mvcx, int mvcy, const int16_t *cand,
-                                     int ncand, int &out_mvx, int &out_mvy, uint32_t &out_cost, MeTeam<TW> &tm) {
+template <class S>
+__device__ void warp_motion_estimate(const S *orig, int os, const S *ref, int rs, MeCtx &c, int mvcx, int mvcy, const int16_t *cand, int ncand, int &out_mvx,
+                                     int &out_mvy, uint32_t &out_cost) {
   const int lane = lane_id();
-  const int band_h = c.height / TW, row0 = tm.warp * band_h;  // this warp's rows
-  const S *orig = orig_full + row0 * os, *ref = ref_full + row0 * rs;
   const int s = c.s, shift = c.bitdepth - 8;
   uint32_t min_sad = 1u << 31;  // MAX_UINT32, common/global.h:63
   int optx = 0, opty = 0;
@@ -860,14 +764,14 @@ __device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_fu
         int base = s * (cx >> 2) + s * (cy >> 2) * rs;
 #pragma unroll
         for (int t = 0; t < 5; t++) {
-          uint32_t v = tm.sum(multi_sad<S, TW>(orig, os, ref, rs, c.width, band_h, base + offs[t], n));
+          uint32_t v = multi_sad<S>(orig, os, ref, rs, c.width, c.height, base + offs[t], n);
           if (v < b) { b = v; bxo = offs[t]; }
         }
         sad = b;
         cx = (int)(int16_t)(cx + (s * bxo << 2));
         c.n_int += 5 * n;
       } else {
-        sad = tm.sum(multi_sad<S, TW>(orig, os, ref, rs, c.width, band_h, s * (cx >> 2) + s * (cy >> 2) * rs, n));
+        sad = multi_sad<S>(orig, os, ref, rs, c.width, c.height, s * (cx >> 2) + s * (cy >> 2) * rs, n);
         c.n_int += n;
       }
       uint32_t cost = (sad >> shift) + mv_cost(c.lambda, quote_mv_bits(cy - c.mvpy, cx - c.mvpx));
@@ -901,14 +805,14 @@ __device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_fu
       int bxo = 0;
 #pragma unroll
       for (int t = 0; t < 5; t++) {
-        uint32_t v = tm.sum(multi_sad<S, TW>(orig, os, ref, rs, c.width, band_h, pos + offs[t], n));
+        uint32_t v = multi_sad<S>(orig, os, ref, rs, c.width, c.height, pos + offs[t], n);
         if (v < b) { b = v; bxo = offs[t]; }
       }
       sad = b;
       cx = (int)(int16_t)(cx + (s * bxo << 2));
       c.n_int += 5 * n;
     } else {
-      sad = tm.sum(multi_sad<S, TW>(orig, os, ref, rs, c.width, band_h, pos, n));
+      sad = multi_sad<S>(orig, os, ref, rs, c.width, c.height, pos, n);
       c.n_int += n;
     }
     uint32_t cost = (sad >> shift) + mv_cost(c.lambda, quote_mv_bits(cy - c.mvpy, cx - c.mvpx));
@@ -934,7 +838,7 @@ __device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_fu
       int dir = (start + lane) % 6;
       int cx = (int)(int16_t)(refx + diy[dir] * 4), cy = (int)(int16_t)(refy + dix[dir] * 4);
       clip_mv(cx, cy, c.ypos, c.xpos, c.fw, c.fh, c.size, c.size, c.sign);
-      uint32_t sad = tm.sum(multi_sad<S, TW>(orig, os, ref, rs, c.width, band_h, s * (cx >> 2) + s * (cy >> 2) * rs, n));
+      uint32_t sad = multi_sad<S>(orig, os, ref, rs, c.width, c.height, s * (cx >> 2) + s * (cy >> 2) * rs, n);
       c.n_int += n;
       uint32_t cost = (sad >> shift) + mv_cost(c.lambda, quote_mv_bits(cy - c.mvpy, cx - c.mvpx));
       uint32_t best;
@@ -969,17 +873,15 @@ __device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_fu
       const int bx = optx, by = opty;
       uint32_t sad = 0xffffffffu;
       if (sizeof(S) == 1 && stage == 0 && !((bx | by) & 3))
-        sad = halfpel_stage_sads_u8((const uint8_t *)orig_full, os, (const uint8_t *)ref_full, rs, c.width, c.height, bx, by, dn, dm, c.sign, c.bip, c.fw, c.fh, c.xpos, c.ypos,
-                                    row0, band_h);
+        sad = halfpel_stage_sads_u8((const uint8_t *)orig, os, (const uint8_t *)ref, rs, c.width, c.height, bx, by, dn, dm, c.sign, c.bip, c.fw, c.fh, c.xpos, c.ypos);
       const int i1 = (lane & 7) + 1;
       const int cy = (int)(int16_t)(by + dm[i1]), cx = (int)(int16_t)(bx + dn[i1]);
       if (sad == 0xffffffffu) {  // 16-bit samples, the quarter-pel stage, or a half-pel geometry the planes do not take: one probe per 4-lane group
         const int tq = (lane >> 2) + 1;
         const int qy = (int)(int16_t)(by + dm[tq]), qx = (int)(int16_t)(bx + dn[tq]);
-        sad = subpel_stage_sads<S>(orig_full, os, ref_full, rs, c.width, c.height, qx, qy, c.sign, c.bip, c.fw, c.fh, c.xpos, c.ypos, c.bitdepth, row0, band_h);
+        sad = subpel_stage_sads<S>(orig, os, ref, rs, c.width, c.height, qx, qy, c.sign, c.bip, c.fw, c.fh, c.xpos, c.ypos, c.bitdepth);
         sad = __shfl_sync(FULL, sad, (lane & 7) * 4);
       }
-      sad = tm.sum(sad);
       const uint32_t cost = (sad >> shift) + mv_cost(c.lambda, quote_mv_bits(cy - c.mvpy, cx - c.mvpx));
       int yd = 0, xd = 0;
       for (int i = 1; i <= 8; i++) {
@@ -999,7 +901,7 @@ __device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_fu
     // ---- bilinear approximations (:664-703)
     int rx = (int)(int16_t)(refx * s), ry = (int)(int16_t)(refy * s);
     int spx, spy;
-    uint32_t sad = warp_sad_fasthalf<S>(orig_full, os, ref_full + (rx >> 2) + (ry >> 2) * rs, rs, c.width, c.height, spx, spy);
+    uint32_t sad = warp_sad_fasthalf<S>(orig, os, ref + (rx >> 2) + (ry >> 2) * rs, rs, c.width, c.height, spx, spy);
     uint32_t cost = (sad >> shift) + mv_cost(c.lambda, quote_mv_bits(ry + s * spy - c.mvpy, rx + s * spx - c.mvpx));
     if (cost < cmin) { cmin = cost; xdh = s * spx; ydh = s * spy; }
     spx = xdh;
@@ -1009,169 +911,9 @@ __device__ void warp_motion_estimate(const S *orig_full, int os, const S *ref_fu
     optx = (int)(int16_t)(optx + xdh);
     opty = (int)(int16_t)(opty + ydh);
     int qx, qy;
-    sad = warp_sad_fastquarter<S>(orig_full, os, ref_full + s * (rx >> 2) + s * (ry >> 2) * rs, rs, c.width, c.height, spx, spy, qx, qy);
+    sad = warp_sad_fastquarter<S>(orig, os, ref + s * (rx >> 2) + s * (ry >> 2) * rs, rs, c.width, c.height, spx, spy, qx, qy);
     cost = (sad >> shift) + mv_cost(c.lambda, quote_mv_bits(ry + s * qy - c.mvpy, rx + s * qx - c.mvpx));
     if (cost < cmin) { cmin = cost; xdq = s * qx; ydq = s * qy; }
-  }
-  out_mvx = (int)(int16_t)(optx + xdq);
-  out_mvy = (int)(int16_t)(opty + ydq);
-  out_cost = cmin < min_sad ? cmin : min_sad;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// a5 for small blocks: FOUR searches per warp, eight lanes each.  A search over a block of <= 64 samples spends most of its
-// instructions in stages that can use only 3-8 lanes (candidate list, hexagon rounds, the eight sub-pel probes) and in per-stage
-// scalar work (clipping, pricing, winner selection); sharing the warp between four searches issues that work once for four.
-// Every lane of a group carries its search's state; all collectives use the group's 8-lane mask, so groups diverge freely.
-// Same stages, visiting order and tie rules as warp_motion_estimate (8-bit samples, speed 0).
-// ---------------------------------------------------------------------------------------------------------------
-struct QuadItem {
-  const uint8_t *orig, *ref;
-  const int16_t *cand;
-  double lambda;
-  int os, rs, size, w, h, sign, xpos, ypos, mvpx, mvpy, mvcx, mvcy, ncand;
-};
-__device__ __forceinline__ int group_first_min(unsigned gm, uint32_t cost, bool valid, uint32_t &best) {  // lowest lane among the minima; -1 if none valid
-  const uint32_t c = valid ? cost : 0xffffffffu;
-  best = __reduce_min_sync(gm, c);
-  const unsigned who = __ballot_sync(gm, valid && c == best);
-  return who ? __ffs(who) - 1 : -1;
-}
-__device__ __noinline__ void quad_motion_estimate(const QuadItem &q, int fw, int fh, int bip, int &out_mvx, int &out_mvy, uint32_t &out_cost, unsigned &n_int) {
-  const int lane = lane_id(), gl = lane & 7, g0 = lane & 24;
-  const unsigned gm = 0xffu << g0;
-  const int s = q.sign ? -1 : 1;
-  uint32_t min_sad = 1u << 31;
-  int optx = 0, opty = 0;
-  int refx = (int)(int16_t)(((q.mvcx + 2) >> 2) << 2), refy = (int)(int16_t)(((q.mvcy + 2) >> 2) << 2);
-  n_int = 0;
-  // SAD + rate of one integer position (this lane's probe)
-  auto int_cost = [&](int cx, int cy, uint32_t &sad_out) {
-    const uint8_t *r = q.ref + s * (cx >> 2) + s * (cy >> 2) * q.rs;
-    sad_out = sad_partial<uint8_t>(q.orig, q.os, r, q.rs, q.w, q.h, 0, 1);
-  };
-  // ---- telescope (:531-561): 25 / 24 grid points per step, eight per pass; a lane keeps its earliest minimum, the group then takes the
-  // smallest cost and, among equal costs, the earliest visiting index
-  for (int step = 32; step >= 4; step >>= 1) {
-    const int n = step < 32 ? 24 : 25;
-    uint32_t bc = 0xffffffffu;
-    int bidx = 64, bx = 0, by = 0;
-    for (int pass = 0; pass < 4; pass++) {
-      const int vi = pass * 8 + gl;
-      if (vi < n) {
-        int idx = vi;
-        if (step < 32 && idx >= 12) idx++;
-        int cx = (int)(int16_t)(refx + (idx % 5 - 2) * step), cy = (int)(int16_t)(refy + (idx / 5 - 2) * step);
-        clip_mv(cx, cy, q.ypos, q.xpos, fw, fh, q.size, q.size, q.sign);
-        uint32_t sad;
-        int_cost(cx, cy, sad);
-        const uint32_t c = sad + mv_cost(q.lambda, quote_mv_bits(cy - q.mvpy, cx - q.mvpx));
-        if (c < bc) { bc = c; bidx = vi; bx = cx; by = cy; }
-      }
-    }
-    n_int += n;
-    const uint32_t m = __reduce_min_sync(gm, bc);
-    const unsigned mi = __reduce_min_sync(gm, bc == m ? (unsigned)bidx : 64u);
-    const unsigned who = __ballot_sync(gm, bc == m && (unsigned)bidx == mi);
-    const int wl = __ffs(who) - 1;
-    const int wx = __shfl_sync(gm, bx, wl), wy = __shfl_sync(gm, by, wl);
-    if (m < min_sad) { min_sad = m; optx = wx; opty = wy; }
-    refx = optx;
-    refy = opty;
-  }
-  // ---- candidates (:564-581); blocks of a 16x16 coding block use the five-position wide SAD
-  for (int base = 0; base < q.ncand; base += 8) {
-    const int n = min(8, q.ncand - base);
-    const bool valid = gl < n;
-    int cx = 0, cy = 0;
-    uint32_t cost = 0;
-    if (valid) {
-      cx = (int)(int16_t)(q.cand[2 * (base + gl)] << 2);
-      cy = (int)(int16_t)(q.cand[2 * (base + gl) + 1] << 2);
-      clip_mv(cx, cy, q.ypos, q.xpos, fw, fh, q.size, q.size, q.sign);
-      uint32_t sad;
-      if (q.size == 16) {
-        const int offs[5] = {-3, -1, 0, 1, 3};
-        const uint8_t *r = q.ref + s * (cx >> 2) + s * (cy >> 2) * q.rs;
-        uint32_t b = 0xffffffffu;
-        int bxo = 0;
-#pragma unroll
-        for (int t = 0; t < 5; t++) {
-          const uint32_t v = sad_partial<uint8_t>(q.orig, q.os, r + offs[t], q.rs, q.w, q.h, 0, 1);
-          if (v < b) { b = v; bxo = offs[t]; }
-        }
-        sad = b;
-        cx = (int)(int16_t)(cx + (s * bxo << 2));
-      } else
-        int_cost(cx, cy, sad);
-      cost = sad + mv_cost(q.lambda, quote_mv_bits(cy - q.mvpy, cx - q.mvpx));
-    }
-    n_int += (q.size == 16 ? 5 : 1) * n;
-    uint32_t best;
-    const int wl = group_first_min(gm, cost, valid, best);
-    const int wx = __shfl_sync(gm, cx, wl < 0 ? g0 : wl), wy = __shfl_sync(gm, cy, wl < 0 ? g0 : wl);
-    if (wl >= 0 && best < min_sad) { min_sad = best; optx = wx; opty = wy; }
-  }
-  refx = optx;
-  refy = opty;
-  // ---- hexagon refinement (:583-616)
-  {
-    int start = 0, end = 5;
-    for (int step = 1; step < 6; step++) {
-      const int diy[6] = {1, 2, 1, -1, -2, -1}, dix[6] = {-1, 0, 1, 1, 0, -1};
-      const int n = ((end - start + 6) % 6) + 1;
-      const bool valid = gl < n;
-      const int dir = (start + gl) % 6;
-      int cx = (int)(int16_t)(refx + diy[dir] * 4), cy = (int)(int16_t)(refy + dix[dir] * 4);
-      uint32_t cost = 0;
-      if (valid) {
-        clip_mv(cx, cy, q.ypos, q.xpos, fw, fh, q.size, q.size, q.sign);
-        uint32_t sad;
-        int_cost(cx, cy, sad);
-        cost = sad + mv_cost(q.lambda, quote_mv_bits(cy - q.mvpy, cx - q.mvpx));
-      }
-      n_int += n;
-      uint32_t best;
-      const int wl = group_first_min(gm, cost, valid, best);
-      const int wx = __shfl_sync(gm, cx, wl), wy = __shfl_sync(gm, cy, wl);
-      int best_dir = -1;
-      if (best < min_sad) { min_sad = best; optx = wx; opty = wy; best_dir = (start + (wl - g0)) % 6; }
-      refx = optx;
-      refy = opty;
-      start = best_dir ? best_dir - 1 : 5;
-      end = start + 2;
-      end -= (end >= 6) * 6;
-      if (best_dir < 0) break;
-    }
-  }
-  // ---- half-pel, then quarter-pel probes (:625-663): probe i on lane i - 1 of the group
-  int ydh = 0, xdh = 0, ydq = 0, xdq = 0;
-  uint32_t cmin = min_sad;
-  for (int stage = 0; stage < 2; stage++) {
-    const int8_t *dm = stage ? c_qm : c_hm, *dn = stage ? c_qn : c_hn;
-    const int cy = (int)(int16_t)(opty + dm[gl + 1]), cx = (int)(int16_t)(optx + dn[gl + 1]);
-    int hi, vi, xf, yf;
-    split_mv(cx, cy, q.sign, 2, fw, fh, q.xpos, q.ypos, q.w, q.h, hi, vi, xf, yf);
-    const uint8_t *ip = q.ref + vi * q.rs + hi;
-    const int RH = q.h >= 8 ? 8 : q.h, nseg = q.h / RH, units = (q.w >> 2) * nseg;
-    uint32_t sad = 0;
-    for (int u = 0; u < units; u++) {
-      const int strip = u / nseg, seg = u - strip * nseg;
-      sad += strip_sad_subpel_u8(q.orig, q.os, ip, q.rs, strip * 4, seg * RH, RH, xf, yf, bip);
-    }
-    const uint32_t cost = sad + mv_cost(q.lambda, quote_mv_bits(cy - q.mvpy, cx - q.mvpx));
-    int yd = 0, xd = 0;
-    for (int i = 1; i <= 8; i++) {
-      const uint32_t ci = __shfl_sync(gm, cost, g0 + i - 1);
-      if (ci < cmin) { cmin = ci; yd = dm[i]; xd = dn[i]; }
-    }
-    if (stage == 0) {
-      ydh = yd; xdh = xd;
-      optx = (int)(int16_t)(optx + xdh);
-      opty = (int)(int16_t)(opty + ydh);
-    } else {
-      ydq = yd; xdq = xd;
-    }
   }
   out_mvx = (int)(int16_t)(optx + xdq);
   out_mvy = (int)(int16_t)(opty + ydq);

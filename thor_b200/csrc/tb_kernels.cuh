@@ -59,160 +59,29 @@ __global__ void fast_subpel_kernel(const S *a, int as, const S *b, int bs, int w
 }
 
 // ---- a5 --------------------------------------------------------------------------------------------------------
-// Scheduling of a search batch.  Searches cost ~ area x probes and a batch mixes 4x4 ... 128x128 blocks; a single warp needs
-// milliseconds for one 128x128 search.  So blocks of >= 2048 samples are searched by the whole CTA (four warps on four row
-// bands, MeTeam), which divides their latency by four: a counting sort (three tiny kernels: histogram, scan, scatter) lists
-// them largest first, and one persistent kernel first draws from that list with an atomic cursor (longest-processing-time
-// first), then draws the remaining searches, one warp each, from the caller's array in its own order.
-// class = ilog2(area), + 16 when the CTA-team form applies (speed 0, height a multiple of 8 rows per warp)
-constexpr int ME_TEAM_WARPS = WARPS_PER_CTA;
-constexpr int ME_DRAW = 4;
-__device__ __forceinline__ int me_class(int w, int h, int speed) {
-  const int area = w * h, b = min(ilog2(max(area, 1)), 15);
-  return (speed == 0 && area >= 2048 && (h % (8 * ME_TEAM_WARPS)) == 0) ? 16 + b : b;
-}
-// meta layout (ints): [0,32) histogram, [32,64) first list position of each class, [64,96) fill cursors, 96 = number of team
-// items, 97 = team cursor, 98 = warp cursor, 99 = number of listed items, 100 = group cursor.  A class functor returns the
-// class (0..31; >= 16: searched by the whole CTA) of an item, or -1 when the item is not listed.
-struct MeClassOf {
-  int speed, quad;  // quad: 8-bit samples and speed 0 -> blocks of <= 64 samples are listed too (class 1) and searched four per warp
-  __device__ __forceinline__ int operator()(const tb_me_item_t &q) const {
-    const int c = me_class(q.width, q.height, speed);
-    if (c >= 16) return c;  // team items, largest first
-    if (quad && (int)q.width * (int)q.height <= 64 && !((q.width | q.height) & 3) && !(q.ostride & 3) && !(q.rstride & 3) &&
-        !((uintptr_t)q.orig & 3))
-      return 1;
-    return -1;  // the others are drawn from the caller's array in its own order
-  }
-};
-template <class Item, class F> __global__ void sched_hist_kernel(const Item *items, int n, F f, int *meta) {
-  __shared__ int h[32];
-  if (threadIdx.x < 32) h[threadIdx.x] = 0;
-  __syncthreads();
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const int c = f(items[i]);
-    if (c >= 0) atomicAdd(&h[c], 1);
-  }
-  __syncthreads();
-  if (threadIdx.x < 32 && h[threadIdx.x]) atomicAdd(&meta[threadIdx.x], h[threadIdx.x]);
-}
-__global__ void sched_scan_kernel(int *meta) {
-  const int b = threadIdx.x;  // 32 threads
-  int before = 0, team = 0, all = 0;
-  for (int k = 31; k > b; k--) before += meta[k];
-  for (int k = 0; k < 32; k++) { all += meta[k]; if (k >= 16) team += meta[k]; }
-  meta[32 + b] = before;
-  meta[64 + b] = 0;
-  if (b == 0) { meta[96] = team; meta[97] = 0; meta[98] = 0; meta[99] = all; meta[100] = 0; }
-}
-template <class Item, class F> __global__ void sched_scatter_kernel(const Item *items, int n, F f, int *meta, int *idx) {
-  // warp-aggregated: the lanes of a warp that hold the same class reserve their list positions with ONE atomic
-  const int nround = (n + gridDim.x * blockDim.x - 1) / (gridDim.x * blockDim.x);
-  for (int k = 0; k < nround; k++) {
-    const int i = (k * gridDim.x + blockIdx.x) * blockDim.x + threadIdx.x;
-    const int c = i < n ? f(items[i]) : -1;
-    const unsigned peers = __match_any_sync(FULL, c);
-    int base = 0;
-    const int leader = __ffs(peers) - 1;
-    if (c >= 0 && lane_id() == leader) base = atomicAdd(&meta[64 + c], __popc(peers));
-    base = __shfl_sync(FULL, base, leader);
-    if (c >= 0) idx[meta[32 + c] + base + __popc(peers & ((1u << lane_id()) - 1))] = i;
-  }
-}
-
-template <class S, int TW>
-__device__ __noinline__ void me_run_item(const tb_me_item_t *items, int it, const int16_t *cand, int bitdepth, int speed, int bip, int fw, int fh, tb_me_result_t *out,
-                                            unsigned long long *stats, MeTeam<TW> &tm) {
-  tb_me_item_t q = items[it];
-  MeCtx c;
-  c.size = q.size; c.width = q.width; c.height = q.height; c.sign = q.sign; c.s = q.sign ? -1 : 1;
-  c.xpos = q.xpos; c.ypos = q.ypos; c.fw = fw; c.fh = fh; c.bitdepth = bitdepth; c.speed = speed; c.bip = bip;
-  c.mvpx = q.mvp_x; c.mvpy = q.mvp_y; c.lambda = q.lambda; c.n_int = 0; c.n_sub = 0;
-  int mx, my;
-  uint32_t cost;
-  warp_motion_estimate<S, TW>((const S *)q.orig, q.ostride, (const S *)q.ref, q.rstride, c, q.mvc_x, q.mvc_y, cand + 2 * (size_t)q.cand_ofs, q.ncand, mx, my, cost, tm);
-  if (lane_id() == 0 && tm.warp == 0) {
-    out[it].mvx = (int16_t)mx; out[it].mvy = (int16_t)my; out[it].cost = cost;
-    if (stats) {  // roofline accounting (SURVEY.md §8d): samples compared at integer positions, samples fetched for sub-pel probes
-      atomicAdd(&stats[0], 1ull);
-      atomicAdd(&stats[1], (unsigned long long)c.n_int);
-      atomicAdd(&stats[2], (unsigned long long)c.n_sub);
-      atomicAdd(&stats[3], (unsigned long long)(c.n_int + 1) * q.width * q.height);
-      atomicAdd(&stats[4], (unsigned long long)c.n_sub * ((q.width + 5) * (q.height + 5) + q.width * q.height));
-    }
-  }
-}
-
+// One warp per search, grid-stride over the caller's array in its order (neighbouring items share samples: they run on
+// neighbouring warps).  The search is warp_motion_estimate, the routine of the device RD loop.
 template <class S>
-__global__ void __launch_bounds__(CTA_THREADS, ME_MINBLOCKS) me_batch_kernel(const tb_me_item_t *items, int n, const int *idx, int *meta, const int16_t *cand, int bitdepth,
-                                                                                 int speed, int bip, int fw, int fh, tb_me_result_t *out, unsigned long long *stats) {
-  __shared__ uint32_t xch[2 * ME_TEAM_WARPS * 32];
-  __shared__ int s_next;
-  const int nteam = meta[96], nlisted = meta[99];
-  const int quad = sizeof(S) == 1 && speed == 0;
-  // phase 1: the CTA as a team on the large blocks
-  {
-    MeTeam<ME_TEAM_WARPS> tm;
-    tm.xch = xch; tm.warp = threadIdx.x >> 5; tm.phase = 0;
-    for (;;) {
-      if (threadIdx.x == 0) s_next = atomicAdd(&meta[97], 1);
-      __syncthreads();
-      const int k = s_next;
-      __syncthreads();
-      if (k >= nteam) break;
-      me_run_item<S, ME_TEAM_WARPS>(items, idx[k], cand, bitdepth, speed, bip, fw, fh, out, stats, tm);
-    }
-  }
-  // phase 2: the searches that are neither team nor quad items, one warp each, drawn four at a time from the caller's array
-  // (neighbouring items share samples: keep them on neighbouring warps)
-  const MeClassOf cls{speed, quad};
-  {
-    MeTeam<1> tm;
-    tm.xch = nullptr; tm.warp = 0; tm.phase = 0;
-    for (;;) {
-      int k = 0;
-      if (lane_id() == 0) k = atomicAdd(&meta[100], ME_DRAW);
-      k = __shfl_sync(FULL, k, 0);
-      if (k >= n) break;
-      for (int it = k; it < min(k + ME_DRAW, n); it++) {
-        if (nlisted && cls(items[it]) >= 0) continue;
-        me_run_item<S, 1>(items, it, cand, bitdepth, speed, bip, fw, fh, out, stats, tm);
+__global__ void __launch_bounds__(CTA_THREADS, ME_MINBLOCKS) me_batch_kernel(const tb_me_item_t *items, int n, const int16_t *cand, int bitdepth, int speed, int bip, int fw,
+                                                                             int fh, tb_me_result_t *out, unsigned long long *stats) {
+  for (int it = global_warp(); it < n; it += total_warps()) {
+    tb_me_item_t q = items[it];
+    MeCtx c;
+    c.size = q.size; c.width = q.width; c.height = q.height; c.sign = q.sign; c.s = q.sign ? -1 : 1;
+    c.xpos = q.xpos; c.ypos = q.ypos; c.fw = fw; c.fh = fh; c.bitdepth = bitdepth; c.speed = speed; c.bip = bip;
+    c.mvpx = q.mvp_x; c.mvpy = q.mvp_y; c.lambda = q.lambda; c.n_int = 0; c.n_sub = 0;
+    int mx, my;
+    uint32_t cost;
+    warp_motion_estimate<S>((const S *)q.orig, q.ostride, (const S *)q.ref, q.rstride, c, q.mvc_x, q.mvc_y, cand + 2 * (size_t)q.cand_ofs, q.ncand, mx, my, cost);
+    if (lane_id() == 0) {
+      out[it].mvx = (int16_t)mx; out[it].mvy = (int16_t)my; out[it].cost = cost;
+      if (stats) {  // roofline accounting (SURVEY.md §8d): samples compared at integer positions, samples fetched for sub-pel probes
+        atomicAdd(&stats[0], 1ull);
+        atomicAdd(&stats[1], (unsigned long long)c.n_int);
+        atomicAdd(&stats[2], (unsigned long long)c.n_sub);
+        atomicAdd(&stats[3], (unsigned long long)(c.n_int + 1) * q.width * q.height);
+        atomicAdd(&stats[4], (unsigned long long)c.n_sub * ((q.width + 5) * (q.height + 5) + q.width * q.height));
       }
-    }
-  }
-  // phase 3: the listed small blocks (8-bit, <= 64 samples), four per warp (quad_motion_estimate).  They come last: the launch
-  // ends on its cheapest searches, and the two code paths do not alternate in the instruction cache.
-  if (sizeof(S) == 1) {
-    const int nsmall = nlisted - nteam;
-    for (;;) {
-      int k = 0;
-      if (lane_id() == 0) k = atomicAdd(&meta[98], 4);
-      k = __shfl_sync(FULL, k, 0);
-      if (k >= nsmall) break;
-      const int slot = k + (lane_id() >> 3);
-      if (slot < nsmall) {
-        const int mine = idx[nteam + slot];
-        const tb_me_item_t q = items[mine];
-        QuadItem qi;
-        qi.orig = (const uint8_t *)q.orig; qi.ref = (const uint8_t *)q.ref; qi.cand = cand + 2 * (size_t)q.cand_ofs; qi.lambda = q.lambda;
-        qi.os = q.ostride; qi.rs = q.rstride; qi.size = q.size; qi.w = q.width; qi.h = q.height; qi.sign = q.sign; qi.xpos = q.xpos; qi.ypos = q.ypos;
-        qi.mvpx = q.mvp_x; qi.mvpy = q.mvp_y; qi.mvcx = q.mvc_x; qi.mvcy = q.mvc_y; qi.ncand = q.ncand;
-        int mx, my;
-        uint32_t cost;
-        unsigned n_int;
-        quad_motion_estimate(qi, fw, fh, bip, mx, my, cost, n_int);
-        if ((lane_id() & 7) == 0) {
-          out[mine].mvx = (int16_t)mx; out[mine].mvy = (int16_t)my; out[mine].cost = cost;
-          if (stats) {
-            atomicAdd(&stats[0], 1ull);
-            atomicAdd(&stats[1], (unsigned long long)n_int);
-            atomicAdd(&stats[2], 16ull);
-            atomicAdd(&stats[3], (unsigned long long)(n_int + 1) * q.width * q.height);
-            atomicAdd(&stats[4], 16ull * ((q.width + 5) * (q.height + 5) + q.width * q.height));
-          }
-        }
-      }
-      __syncwarp();
     }
   }
 }

@@ -19,7 +19,6 @@
 #define TB_LDF(p) __ldcg(p)
 #define TB_ROLL _Pragma("unroll 1")  // loops stay loops: the kernel is bound by instruction fetch, not by loop overhead
 #define TB_ME_STAGE_PROF 1  // cycles per search stage (telescope, candidates, hexagon, half-pel, quarter-pel) of blocks <= 16 in the kernel's counters
-#define TB_SAD_ROWS 1  // integer-position SADs of blocks >= 32 bytes wide: lanes along the row (multi_sad_rows)
 #define tb tb_rdo_tu
 #include <cstdio>
 #include <cstdlib>
@@ -337,11 +336,9 @@ template <class S> struct DevBackend {
     c.size = size; c.width = w; c.height = h; c.sign = sign; c.s = sign ? -1 : 1; c.xpos = xpos; c.ypos = ypos; c.fw = F->width; c.fh = F->height;
     c.bitdepth = F->bitdepth; c.speed = F->speed; c.bip = F->enable_bipred; c.mvpx = mvp.x; c.mvpy = mvp.y; c.lambda = lambda; c.n_int = 0; c.n_sub = 0;
     for (int k = 0; k < 5; k++) c.cyc[k] = 0;
-    MeTeam<1> tm;
-    tm.xch = nullptr; tm.warp = 0; tm.phase = 0;
     int mx, my;
     uint32_t cost;
-    warp_motion_estimate<S, 1>(org, os, ref, rs, c, mvc.x, mvc.y, (const int16_t *)cand, ncand, mx, my, cost, tm);
+    warp_motion_estimate<S>(org, os, ref, rs, c, mvc.x, mvc.y, (const int16_t *)cand, ncand, mx, my, cost);
     mx = __shfl_sync(FULL, mx, 0); my = __shfl_sync(FULL, my, 0); cost = __shfl_sync(FULL, cost, 0);
     mv->x = (int16_t)mx; mv->y = (int16_t)my;
     if (lane() == 0) {
