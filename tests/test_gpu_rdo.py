@@ -8,7 +8,7 @@ import subprocess
 import pytest
 
 from test_dropin_link import HDB, LDB, REF, synth_yuv
-from test_rdo_matrix import hard_yuv
+from test_rdo_matrix import BENCH_HDB, BENCH_HDB16, hard_yuv
 
 needs = pytest.mark.skipif(not (os.path.exists(os.path.join(REF, "Thorenc_b200_rdo")) and os.path.exists(os.path.join(REF, "Thorenc"))),
                            reason="oracle/_ref (reference objects + drop-in links) not built")
@@ -52,6 +52,10 @@ CLIPS = {"hdb_10bit_q4_hard": (4, hard_yuv), "hdb_8bit_q51": (51, synth_yuv), "h
     # 8-bit content in 16-bit frames, where the reference's encoder predicts 0 at one-axis fractions (DESIGN.md §5).  Its decoder filters
     # these normally, so it does not reconstruct the encoder's frames: encoder outputs only
     ("hdb_8bit_fb16", HDB + ["-cdef", "0"], 128, 136, 5, ("-frame_bitdepth", "16"), False),
+    # the benchmark's HDB16 (a 16-picture GOP, B frames at four levels) and HDB with an intra period of 8 (I frames 0, 8 and 16, the B frames of a
+    # second segment), CDEF off so that the reference's decoder reads the small frames' streams
+    ("hdb16_10bit", BENCH_HDB16 + ["-cdef", "0"], 256, 136, 17, ("-bitdepth", "10", "-input_bitdepth", "10"), True),
+    ("hdb_8bit_intra_period8", BENCH_HDB + ["-cdef", "0", "-intra_period", "8"], 256, 136, 17, (), True),
 ])
 def test_device_rd_loop_encode_is_bit_exact(tmp_path, name, flags, w, h, n, extra, decode):
     tmp = str(tmp_path)

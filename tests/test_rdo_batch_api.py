@@ -485,3 +485,31 @@ def test_argument_errors_leave_the_batch_working(lib, golden, pinned):
         batch.round(hosts)
         assert_last_launch(batch, hosts, "after the errors")
     assert_reference(hosts, "after the errors, all three slots")
+
+
+@pytest.mark.parametrize("width", [120, 88, 8])
+def test_16bit_frame_widths_off_the_multiple_of_16_are_refused(lib, golden, pinned, width):
+    """16-bit frames whose width is 8 mod 16: chroma widths of 4 mod 8, which the reference's SIMD chroma interpolation predicts unlike its C code in
+    rectangular frame-edge blocks.  tb_rdo_batch_upload and tb_rdo_encode_frames refuse them with TB_ERR_ARG and a message, and the batch still
+    decides the frames it holds afterwards.  The width is narrowed in a copy of the descriptor of a 128-wide frame (the other checks on it still
+    pass): nothing of that frame reaches the device."""
+    from thor_b200 import rdo_jobs as RJ
+    hosts = frames(golden("hdb_hard_q4_10bit")[:2], pinned)
+    odd = RJ.RdoFrame.from_buffer_copy(bytes(hosts[1].desc))
+    odd.width = width
+    lib.tb_rdo_encode_frames.argtypes = [C.c_void_p, C.c_int]
+    with Batch(lib, 2, 2) as batch:
+        batch.upload(0, hosts[0])
+        assert lib.tb_rdo_batch_upload(batch.b, 1, C.byref(odd)) == TB_ERR_ARG
+        assert b"multiples of 16" in lib.tb_rdo_last_error(), lib.tb_rdo_last_error()
+        assert lib.tb_rdo_batch_run(batch.b, 2) == TB_ERR_ARG, "slot 1 was never uploaded"
+        descs = (RJ.RdoFrame * 2)(hosts[0].desc, odd)
+        assert lib.tb_rdo_encode_frames(descs, 2) == TB_ERR_ARG
+        assert b"multiples of 16" in lib.tb_rdo_last_error(), lib.tb_rdo_last_error()
+        batch.upload(1, hosts[1])
+        batch.run(2)
+        for s, hf in enumerate(hosts):
+            batch.download(s, hf)
+        batch.sync()
+        assert_last_launch(batch, hosts, "after the refused uploads")
+    assert_reference(hosts, "after the refused uploads")

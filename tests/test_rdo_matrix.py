@@ -2,7 +2,7 @@
 
 One table of cases (CASES) drives every test here:
   CPU  oracle/_ref/Thorenc_rdocheck with TB_RDO_VERIFY=1: every super block of every case, decided by thor_b200/csrc/tb_rdo.h over the plain-C
-       oracle and by the reference's process_block() on the same encoder state, must be identical; five cases also run with eight simulated warps.
+       oracle and by the reference's process_block() on the same encoder state, must be identical; nine cases also run with eight simulated warps.
   GPU  every case captured with the reference (oracle/_ref/Thorenc_capture); all 8-bit frames of all cases decided in ONE tb_rdo_encode_frames()
        launch, the 8-bit frames held in 16-bit samples (-frame_bitdepth 16) in a second, all 10-bit frames in a third, all 12-bit frames in a
        fourth.  Frames of one launch differ in size, qp, speed, options and (8 bits) super-block size.  Every
@@ -27,6 +27,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 
+import bench
 from test_dropin_link import HDB, LDB, REF, synth_yuv
 
 
@@ -82,6 +83,8 @@ CONTENT = {"synth": synth_yuv, "hard": hard_yuv, "pan_neg": pan_yuv, "pan_pos": 
 HDB0 = HDB + ["-cdef", "0"]   # tiny frames + CDEF corrupt the reference's header (SURVEY §8c.3)
 FB16 = ["-frame_bitdepth", "16"]   # 16-bit frames; with 8-bit input the internal bit depth stays 8
 SB64 = ["-log2_sb_size", "6"]
+# the benchmark's configurations, CDEF on: the headline HDB, HDB16 (configs[4]) and RA (configs[3], HDB with an intra period)
+BENCH_HDB, BENCH_HDB16, BENCH_RA = (bench.CONFIGS[k][4].split() for k in ("hdb", "hdb10", "ra4k"))
 CASES = [
     # name               flags                                                         w    h    frames qp bitdepth content
     ("hdb_q4",           HDB0,                                                         128, 136, 9, 4,  8,  "synth"),
@@ -134,6 +137,17 @@ CASES = [
     ("ldb_bipred4_s0",   LDB + ["-enable_bipred", "1", "-max_num_ref", "4", "-encoder_speed", "0"], 128, 136, 6, 32, 8, "synth"),
     ("no_cfl_intra",     HDB0 + ["-enable_cfl_intra", "0"],                            128, 136, 5, 32, 8,  "synth"),
     ("no_pb_split",      HDB0 + ["-enable_pb_split", "0"],                             128, 136, 5, 32, 8,  "synth"),
+    # the benchmark's configurations (STRUCTURE has what each case must contain).  HDB16's 16-picture GOP: B frames at four levels, references up
+    # to 13 pictures away.  An intra period of 8: I frames at 8 and 16, B frames of a second segment.  Strips of the 1080p and 2160p frames: 15
+    # and 30 super-block columns (rows wait on their up-right neighbour), the bottom rows of 1080 and 2160 (56 and 112 rows, rectangular
+    # edge blocks 56, 24, 8 and 112, 48, 16 tall), and in RA P frames with up to four references and bi-prediction
+    ("hdb16_10",         BENCH_HDB16,                                                  256, 136, 17, 32, 10, "synth"),
+    ("ra_ip8",           BENCH_HDB + ["-intra_period", "8"],                           256, 136, 17, 32, 8,  "synth"),
+    ("hdb_1080_strip",   BENCH_HDB,                                                    1920, 184, 9, 32, 8,  "synth"),
+    # on synth_yuv at qp 32 the reference codes neither the 112- and 48-row edge blocks nor bi-prediction in RA's P frames (nor 56-row edge
+    # blocks in HDB16's 10-bit P frames); the pans code them
+    ("ra_2160_strip",    BENCH_RA,                                                     3840, 240, 5, 32, 8,  "pan_neg"),
+    ("hdb16_1080_strip_10", BENCH_HDB16,                                               1920, 184, 5, 32, 10, "pan_pos"),
 ]
 BY_NAME = {c[0]: c for c in CASES}
 
@@ -186,7 +200,8 @@ def test_every_super_block_matches_reference_process_block(tmp_path, case):
 
 
 @needs_check
-@pytest.mark.parametrize("name", ["cfl_inter_hard", "hdb_q4_hard_10", "hdb_q51_12", "speed1_hard_12", "hdb_pan_neg", "hdb_sb64_rect", "reorder3_nd"])
+@pytest.mark.parametrize("name", ["cfl_inter_hard", "hdb_q4_hard_10", "hdb_q51_12", "speed1_hard_12", "hdb_pan_neg", "hdb_sb64_rect", "reorder3_nd",
+                                  "hdb16_10", "hdb_1080_strip"])
 def test_overlapped_decision_with_the_device_warp_count(tmp_path, name):
     """the device decides with eight warps per CTA; host threads stand in for them (TBR_HOST_WARPS), see tests/test_rdo_host.py"""
     verify(str(tmp_path), BY_NAME[name], {"TBR_HOST_WARPS": "8"})
@@ -207,19 +222,84 @@ def alloc_into(keep):
 
 
 @pytest.fixture(scope="module")
-def matrix_jobs(tmp_path_factory):
-    """every case captured with the reference encoder: {name: (job directory, jobs)}"""
+def captured_cases(tmp_path_factory):
+    """captured_cases(names) -> {name: (job directory, jobs)}: the cases captured with the reference encoder, each once per module"""
     from test_rdo_jobs import capture
     from thor_b200 import rdo_jobs as RJ
+    done = {}
 
-    def one(case):
-        name, flags, w, h, n, qp, bd, content = case
+    def one(name):
+        _, flags, w, h, n, qp, bd, content = BY_NAME[name]
         d = str(tmp_path_factory.mktemp(name))
         jobdir = capture(d, flags, w, h, n, bd, qp, CONTENT[content])
         return name, (jobdir, RJ.load_jobs(jobdir))
     tmp_path_factory.getbasetemp()  # created lazily: threads that create it at once get different ones, and mktemp then refuses the name
-    with ThreadPoolExecutor(min(8, os.cpu_count() or 1)) as ex:
-        return dict(ex.map(one, CASES))
+
+    def get(names):
+        todo = [n for n in names if n not in done]
+        with ThreadPoolExecutor(max(1, min(8, os.cpu_count() or 1, len(todo)))) as ex:
+            done.update(ex.map(one, todo))
+        return {n: done[n] for n in names}
+    return get
+
+
+@pytest.fixture(scope="module")
+def matrix_jobs(captured_cases):
+    """every case captured with the reference encoder: {name: (job directory, jobs)}"""
+    return captured_cases([c[0] for c in CASES])
+
+
+def edge_heights(job):
+    """the heights inside the picture (height - ypos) of the blocks the reference coded across the picture's bottom edge, from its block state"""
+    h, w = job.hdr.height, job.hdr.width
+    blk = job.blk.reshape(h // 4, w // 4)
+    out = set()
+    for r in range(h // 4):
+        for s in np.unique(blk["size"][r]).tolist():
+            ypos = 4 * r // s * s
+            if ypos + s > h:
+                out.add(h - ypos)
+    return out
+
+
+def structure(name, jobs):
+    """what a case of the benchmark's configurations exists for, from its captured jobs and the reference's decisions in them: a list of what is
+    missing (empty when the case has it all)"""
+    I, P, B = 0, 1, 2
+    nsbx = -(-jobs[0].hdr.width // (1 << jobs[0].hdr.log2_sb_size))
+    missing = []
+    if name == "hdb16_10":
+        levels = {j.hdr.qp for j in jobs if j.hdr.frame_type == B}
+        if len(levels) < 4:
+            missing.append("B frames at four qp levels: %s" % sorted(levels))
+    if name == "ra_ip8":
+        intra = {j.frame_num for j in jobs if j.hdr.frame_type == I}
+        if not {8, 16} <= intra:
+            missing.append("I frames 8 and 16: %s" % sorted(intra))
+    edges = {"hdb_1080_strip": {56, 24, 8}, "hdb16_1080_strip_10": {56, 24, 8}, "ra_2160_strip": {112, 48, 16}}.get(name)
+    if edges:
+        if nsbx != (30 if name == "ra_2160_strip" else 15):
+            missing.append("super-block columns: %d" % nsbx)
+        seen = set().union(*[edge_heights(j) for j in jobs if j.hdr.frame_type != I])
+        if not edges <= seen:
+            missing.append("blocks across the bottom edge %s rows tall: %s" % (sorted(edges), sorted(seen)))
+    if name == "ra_2160_strip":
+        p4 = [j for j in jobs if j.hdr.frame_type == P and j.hdr.num_ref == 4]
+        if not p4:
+            missing.append("a P frame with four references")
+        if not any((j.blk["bipred_flag"] == 2).any() for j in p4):
+            missing.append("bi-prediction in a P frame with four references")
+    return missing
+
+
+STRUCTURE = ["hdb16_10", "ra_ip8", "hdb_1080_strip", "ra_2160_strip", "hdb16_1080_strip_10"]
+
+
+@needs_capture
+@pytest.mark.parametrize("name", STRUCTURE)
+def test_bench_configuration_cases_contain_what_they_exist_for(captured_cases, name):
+    jobs = captured_cases([name])[name][1]
+    assert not structure(name, jobs), structure(name, jobs)
 
 
 @pytest.fixture(scope="module")
@@ -250,6 +330,7 @@ def launches(matrix_jobs):
 def test_matrix_in_one_launch_equals_reference_decisions(launches, key):
     rc, hosts, err = launches(key)
     assert rc == 0, err
+    assert {n for n, _ in hosts} == {c[0] for c in CASES if launch_key(c) == key}   # every case of that sample size and bit depth is in the launch
     assert len({(hf.job.hdr.width, hf.job.hdr.height, hf.job.hdr.qp, hf.job.hdr.encoder_speed) for _, hf in hosts}) > 1  # parameters differ within the launch
     bad = [(name, hf.job.frame_num, r) for name, hf in hosts for r in [hf.check()] if not all(r.values())]
     assert not bad, "%d of %d frames differ from the reference: %s" % (len(bad), len(hosts), bad[:8])

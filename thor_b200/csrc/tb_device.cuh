@@ -114,7 +114,8 @@ __device__ __noinline__ uint32_t multi_sad_narrow(const S *o, int os, const S *r
   constexpr int PW = Word<S>::PW;
   const int lane = lane_id();
   const int nwords = (w / PW) * h;
-  int L = nwords >= 512 ? 32 : (nwords <= 16 ? 1 : nwords >> 4);  // power of two
+  // a power of two (lane groups, group_sum): heights of rectangular frame-edge blocks (12, 24, 28, 56 ...) give other word counts
+  int L = nwords >= 512 ? 32 : (nwords <= 16 ? 1 : 1 << ilog2(nwords >> 4));
   if (L > h) L = h;  // rows are dealt to lanes
   // few positions (hexagon rounds: 3-6, candidate lists): widen the lane group per position while everything still fits one pass
   while (L < 32 && 2 * L * n <= 32 && 2 * L <= h) L *= 2;

@@ -688,6 +688,11 @@ int check_desc(const tb_rdo_frame_t *f) {
              f ? f->num_ref : 0, f ? f->log2_sb_size : 0, f ? f->interp_ref : 0, f ? f->qp : 0, f ? f->ref_pad : 0);
     return TB_ERR_ARG;
   }
+  // the reference's SIMD chroma interpolation of 16-bit samples treats chroma widths of 4 mod 8 unlike its C code, in rectangular frame-edge blocks
+  if (f->sample_bytes == 2 && (f->width & 15)) {
+    snprintf(g_err, sizeof(g_err), "unsupported frame description: 16-bit frames %d wide (16-bit frame widths must be multiples of 16)", f->width);
+    return TB_ERR_ARG;
+  }
   return TB_OK;
 }
 
